@@ -3,6 +3,7 @@
 gcbf/algo/gcbf.py:158-226) on synthetic BASELINE.json configs.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config C3] [--also C2,...|none] [--impl own|reference]
+                    [--dump-outputs DIR]
 
 Workload     : `value` / `e2e` / `roofline` are measured on --config, by default C3 (DubinsCar n=1024, obs=32, B=64 per GPU) -- the
                largest single-GPU configuration of BASELINE.json.  `config.also` carries the same device-timed and end-to-end
@@ -10,7 +11,7 @@ Workload     : `value` / `e2e` / `roofline` are measured on --config, by default
                configurations BASELINE.json defines over 8 GPUs -- C4 (SimpleDrone n=1024, 16 replicas = 2 per GPU) and C5
                (DubinsCar n=4096 dense, 8 graphs = 1 per GPU, gradient all-reduce).
 
-own arm      : gcbf_b200 (sm_100a kernels through the C ABI).  `value` = device-timed throughput with the batch
+own arm      : gcbf_b200 (sm_90a kernels through the C ABI).  `value` = device-timed throughput with the batch
                resident in HBM; `e2e` = the same step driven from pinned HOST buffers (H2D of the states, graph
                build, train step, D2H of the scalars) per step.
 reference arm: the reference algorithm on the host CPU cores.  The reference is pure Python on torch_geometric, which
@@ -18,7 +19,8 @@ reference arm: the reference algorithm on the host CPU cores.  The reference is 
                bit-for-bit against the reference in the build container) -- kind "port".
 Multi-GPU    : one process per GPU (torchrun), environment-parallel: every rank trains on its own B graphs (weak
                scaling), one NCCL all-reduce of the flat gradient bucket per step.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes what the last timed train step of --config returned (h, actions,
+losses, ...) as DIR/<name>.npy: the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -47,7 +49,8 @@ def read_peaks():
             p = json.load(f)
         return dict(hbm_gbs=p['hbm_gbs'], bf16_tflops=p['bf16_tflops'], bf16_sustained=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    # NVIDIA's H100 SXM data sheet (700 W card), dense fp16 / bf16: a bound, not a measured rate
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0, source='H100 SXM data sheet (not measured)')
 
 
 class ClockSampler:
@@ -176,6 +179,8 @@ def measure(cfg_name, args, dev, rank, world, dist, with_roofline, sampler=None)
     ev1.record()
     barrier()
     ms = ev0.elapsed_time(ev1)
+    # the step's results are views into its workspace: copy them out before any later step overwrites them
+    outputs = {k: v.detach().cpu().clone() for k, v in res.items() if torch.is_tensor(v)} if args.dump_outputs and with_roofline else None
     launches = _C.kernel_launches()
     clocks = sampler.stop() if sampler is not None else None
     scal = res['scalars'].tolist()
@@ -244,7 +249,7 @@ def measure(cfg_name, args, dev, rank, world, dist, with_roofline, sampler=None)
         dist.all_reduce(et)
     del algo, data
     return dict(sb=sb, B=B, n=n, E=E, E_total=int(et.item()), ms=ms, ms_e2e=ms_e2e, e2e_runs=e2e_runs, h2d=h2d, launches=launches, clocks=clocks,
-                scal=scal, gemm=gemm, ms_instr=ms_instr)
+                scal=scal, gemm=gemm, ms_instr=ms_instr, outputs=outputs)
 
 
 def rollout_leg(cfg_name, dev, steps=20):
@@ -294,21 +299,6 @@ def controller_leg(cfg_name, dev, calls=5):
             'wall_ms_per_call': round(wall, 3), 'adam_rounds': rounds, 'wall_ms_per_round': round(per_round, 3)}
 
 
-def shape_traffic(dom):
-    """DRAM bytes per launch of the dominant launch shape from the committed `ncu --set full` capture of exactly that shape
-    (profiles/r02_gemm_h_ncu_full.json: {"launches": [{"product", "M", "N", "K", "dram_read_bytes", "dram_write_bytes"}, ...]});
-    None when no capture of this shape exists -- never a number taken from a different launch."""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'r02_gemm_h_ncu_full.json')) as f:
-            caps = json.load(f)['launches']
-    except Exception:
-        return None, None
-    for c in caps:
-        if c.get('product') == dom['product'] and (c.get('M'), c.get('N'), c.get('K')) == (dom['M'], dom['N'], dom['K']):
-            return int(c['dram_read_bytes'] + c['dram_write_bytes']), c.get('source', 'profiles/r02_gemm_h_ncu_full.json')
-    return None, None
-
-
 def run_own(args):
     import torch.distributed as dist
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -356,8 +346,8 @@ def run_own(args):
     peaks = read_peaks()
     agents = B * n * world
     value = agents * args.steps / (ms / 1e3)
-    # dominant kernel: gemm_h_kernel (tcgen05 kind::f16).  Peak = measured dense bf16/fp16 tensor throughput inside a long
-    # step (sustained).  `achieved` counts the ALGORITHMIC fp32 FLOPs (2*M*N*K per product); the kernel issues 3 fp16 MMAs
+    # dominant kernel: gemm_h_kernel (wgmma f16).  Peak = dense bf16/fp16 tensor throughput (MEASURED_PEAKS.json when present,
+    # else the data sheet).  `achieved` counts the ALGORITHMIC fp32 FLOPs (2*M*N*K per product); the kernel issues 3 fp16 MMAs
     # per product (hi*hi + hi*lo + lo*hi), so the tensor pipe itself runs at 3x that: `frac_issued`.
     f16_peak = peaks['bf16_sustained']
     achieved_tflops = gemm['flops'] / max(gemm['ms'], 1e-9) / 1e9
@@ -372,12 +362,11 @@ def run_own(args):
                 'instrumented_ms_per_step': round(ms_instr / args.steps, 4),
                 'whole_step_flops': gemm['flops'] / args.steps,
                 'whole_step_frac': round(gemm['flops'] / args.steps / (ms / args.steps) / 1e9 / f16_peak, 4),
-                'instrumented_pass': 'single stream, CUDA-event pair per GEMM / operand-prep launch', 'traffic': None}
+                'instrumented_pass': 'single stream, CUDA-event pair per GEMM / operand-prep launch'}
     dom = gemm.get('dominant')
     if dom:
         # the launch shape that takes the most GEMM time: algorithmic FLOPs and bytes per launch (companions in: 2 planes x
-        # 2 B per element of each operand; fp32 out) against its CUDA-event duration; DRAM traffic only from a committed
-        # `ncu --set full` capture of exactly this launch shape
+        # 2 B per element of each operand; fp32 out) against its CUDA-event duration
         M_, N_, K_ = dom['M'], dom['N'], dom['K']
         out_elems = {'forward': M_ * N_, 'data-grad': M_ * K_, 'weight-grad': N_ * K_}[dom['product']]
         in_elems = {'forward': M_ * K_ + N_ * K_, 'data-grad': M_ * N_ + N_ * K_, 'weight-grad': M_ * N_ + M_ * K_}[dom['product']]
@@ -388,9 +377,6 @@ def run_own(args):
             'flops_per_launch': dom['flops_per_launch'], 'ms_per_launch': round(dom['ms_per_launch'], 4),
             'achieved': round(tf, 1), 'frac': round(tf / f16_peak, 4), 'frac_issued': round(3 * tf / f16_peak, 4),
             'algorithmic_bytes_per_launch': alg_bytes}
-        roofline['traffic'], src = shape_traffic(dom)
-        if src:
-            roofline['traffic_source'] = src
     line = {
         'metric': METRIC, 'value': round(value, 1), 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
         'ms_per_step': round(ms / args.steps, 4), 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
@@ -398,7 +384,7 @@ def run_own(args):
         'config': {'workload': f'{main_cfg}: {sb.env} n={n} obs={sb.num_obs} B={B}/GPU area={sb.area_size}',
                    'agents_per_step': agents, 'edges_per_gpu': E, 'parallelism': f'dp{world}',
                    'l2': 'no flush: per-step working set (>= 0.2 GB of activations per 2048-wide layer + 98 MB weights) '
-                         'exceeds the 126 MB L2',
+                         'exceeds the 50 MB L2',
                    'also': extra},
         'clocks': m['clocks'],
         'e2e': ({'value': round(agents * args.steps / (ms_e2e / 1e3), 1), 'unit': UNIT, 'h2d_bytes_per_step': m['h2d'],
@@ -416,9 +402,35 @@ def run_own(args):
             line['rollout'] = {'error': repr(ex)[:200]}
     if world == 1 and not args.no_cpu_baseline:
         line['cpu_baseline'] = cpu_baseline(main_cfg, budget_s=25.0)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, m['outputs'])
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, outputs):
+    """DIR/<name>.npy per returned tensor, float64 kept, everything else as float32.  Above 64 MB in all, arrays are cut to a
+    fixed, seeded sample of their leading-dimension rows: one index set per leading-dimension size, so row i of every array
+    with that many rows (h, actions, masks, ...) belongs to the same agent."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v.numpy() if v.dtype == torch.float64 else v.float().numpy() for k, v in outputs.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        frac = DUMP_LIMIT / total
+        index = {}
+        for k, a in arrays.items():
+            if a.ndim and a.shape[0] > 1:
+                n = a.shape[0]
+                if n not in index:
+                    index[n] = np.sort(np.random.default_rng(n).choice(n, max(1, int(n * frac)), replace=False))
+                arrays[k] = a[index[n]]
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f'{k}.npy'), a)
 
 
 def cpu_quota():
@@ -558,7 +570,7 @@ def run_macbf(args):
     dev = torch.device('cuda', 0)
     out = {}
     for name in macbf_probe.WORKLOADS:
-        rec, (sb, algo, data) = macbf_probe.measure(name, dev, steps=max(args.steps, 10), warmup=max(args.warmup, 3))
+        rec, (sb, algo, data) = macbf_probe.measure(name, dev, steps=args.steps, warmup=args.warmup)
         if name == 'ref' and not args.no_cpu_baseline:
             host_threads()
             sys.path.insert(0, os.path.join(ROOT, 'oracle'))
@@ -592,7 +604,11 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true', help='skip the host-buffer leg (profiling runs under ncu only)')
     ap.add_argument('--macbf', action='store_true', help='measure the MACBF baseline train step instead (SURVEY 8f-4; single GPU, own arm only)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the results of the last timed train step of --config as DIR/<name>.npy (own arm, default path)')
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == 'reference' or args.macbf):
+        raise SystemExit('--dump-outputs writes the results of the own arm\'s GCBF train step: not available with --impl reference or --macbf')
     if args.impl == 'reference':
         run_reference(args)
     else:

@@ -163,7 +163,7 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
     R.ws.off = mark0;
     if (R.dry) return 0;
     CHAIN_CUDA(cudaMemsetAsync(B.d_states, 0, (size_t)Nn * s * 4, R.st));
-    CHAIN_CALL(gcbf_edge_attr_bwd(d.env.env, B.states_next, s, b.edge_index, E, B.d_ea, B.d_states, R.st));
+    CHAIN_CALL(edge_attr_bwd_ordered(d.env.env, B.states_next, s, b.edge_index, E, Nn, B.d_ea, B.d_states, R.st));
     CHAIN_CALL(gcbf_step_bwd(&cfg, B.d_states, s, B.pass_mask, B.g, R.st));
     agent_adam_kernel<<<grid_m, 256, 0, R.st>>>(B.act, B.m, B.v, B.t, B.g, B.max_val, noise, B.count, M, a, lr, rand);                                  // :301-305
     GCBF_LAUNCH_OK();

@@ -1,4 +1,4 @@
-"""Builds libgcbf_b200.so (sm_100a) in-tree with nvcc.  `python build.py [--force]`."""
+"""Builds libgcbf_b200.so (sm_90a, H100) in-tree with nvcc.  `python build.py [--force]`."""
 import glob
 import os
 import subprocess
@@ -8,7 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT = os.path.join(os.path.dirname(HERE), 'gcbf_b200', 'libgcbf_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-O3', '-std=c++17', '-lineinfo', '-gencode', 'arch=compute_100a,code=sm_100a', '-Xcompiler', '-fPIC',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = ['-O3', '-std=c++17', '-lineinfo'] + ARCH + ['-Xcompiler', '-fPIC',
          '-I', os.path.join(ROOT, 'include'), '-I', HERE]
 
 
@@ -31,10 +32,8 @@ def build(force=False, verbose=True, extra_defs=(), target=None):
     objdir = os.path.join(HERE, 'build' if target == OUT else 'build_' + os.path.basename(target)[:-3])
     os.makedirs(objdir, exist_ok=True)
     defs = list(extra_defs)
-    if os.path.exists(os.path.join(HERE, 'gemm_tcgen05_f16.cu')):
-        defs.append('-DGCBF_WITH_TCGEN05')
-        if '-DGCBF_NO_SETMAXNREG' not in defs:
-            defs.append('-DGCBF_SETMAXNREG')     # 12 warps: producer warpgroup at 40 registers, epilogue warpgroups at 232 (no spills)
+    if os.path.exists(os.path.join(HERE, 'gemm_wgmma_f16.cu')):
+        defs.append('-DGCBF_WITH_WGMMA')
     procs = []
     objs = []
     for src in sources():
@@ -50,13 +49,10 @@ def build(force=False, verbose=True, extra_defs=(), target=None):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError('nvcc failed')
-    cmd = [NVCC, '-shared', '-o', target] + objs
+    cmd = [NVCC, '-shared'] + ARCH + ['-o', target] + objs
     subprocess.check_call(cmd)
     return target
 
 
 if __name__ == '__main__':
-    if '--epi16' in sys.argv:     # experiment build: 16 promotion / epilogue warps (measured slower) -> load with GCBF_B200_LIB=...
-        print(build(force=True, extra_defs=['-DGCBF_EPI_WARPS=16'], target=OUT.replace('.so', '_epi16.so')))
-    else:
-        print(build(force='--force' in sys.argv))
+    print(build(force='--force' in sys.argv))

@@ -48,7 +48,7 @@ struct Run {
   } while (0)
 #define CHAIN_CUDA(expr) GCBF_CUDA_OK(expr)
 
-// fp16 [hi | lo] companion of an fp32 matrix (gemm_tcgen05_f16.cu)
+// fp16 [hi | lo] companion of an fp32 matrix (gemm_wgmma_f16.cu)
 struct H16 {
   void* buf; const void* amax; int ld, rows, cols;
   int sr, sc;   // strides (words) of the amax array per 128-row block / 256-column tile; 0, 0 = one word per tensor

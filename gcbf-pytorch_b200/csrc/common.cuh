@@ -1,4 +1,4 @@
-// Shared helpers for libgcbf_b200 (sm_100a).  Error reporting, launch checks, warp reductions.
+// Shared helpers for libgcbf_b200 (sm_90a).  Error reporting, launch checks, warp reductions.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,6 +11,16 @@ namespace gcbf {
 void set_error(const char* fmt, ...);
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// Stream-ordered scratch for per-block partial results, and their sum in a fixed order (reduce.cu):
+// target[r * ldt + c] = (accumulate ? target[r * ldt + c] : 0) + part[0][r][c] + part[1][r][c] + ...   (parts of rows x cols each)
+cudaError_t scratch_alloc(void** p, size_t bytes, cudaStream_t st);
+cudaError_t scratch_free(void* p, cudaStream_t st);
+cudaError_t add_partials(const float* part, int parts, int rows, int cols, float* target, int ldt, int accumulate, cudaStream_t st);
+
+// d_states += the VJP of edge_attr like gcbf_edge_attr_bwd, summed in a fixed order (graph.cu); needs the batch's node count
+int edge_attr_bwd_ordered(int env, const float* states, int ld_state, const int64_t* edge_index, int64_t num_edges, int num_nodes,
+                          const float* d_edge_attr, float* d_states, cudaStream_t st);
 
 // in-place single-block exclusive scan of `count` int32 values, data[count] <- total (graph.cu; shared with macbf.cu)
 cudaError_t exclusive_scan_i32(int32_t* data, int count, cudaStream_t st);
@@ -34,7 +44,7 @@ cudaError_t exclusive_scan_i32(int32_t* data, int count, cudaStream_t st);
 
 #define GCBF_LAUNCH_OK() GCBF_CUDA_OK(cudaGetLastError())
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

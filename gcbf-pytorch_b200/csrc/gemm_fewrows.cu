@@ -1,6 +1,6 @@
 // Linear layers with FEW ROWS (M <= 64): the rollout-time forward of a single graph (reference gcbf/algo/gcbf.py:128-139: 16 agents,
 // ~45 edges per env step) and the plumbing config C1.  With so few rows a layer is a stream over its WEIGHTS (2048 x 2048 fp32 = 16 MB,
-// resident in the 126 MB L2 from one pass to the next), not a GEMM tile problem: a 128 x 128 tile grid puts 16 CTAs on 148 SMs.
+// resident in the 50 MB L2 from one pass to the next), not a GEMM tile problem: a 128 x 128 tile grid puts 16 CTAs on 132 SMs.
 //   fwd   : Y[M,N]   = act(alpha * X W^T + b)      warp = 2 output columns, lanes split K (16-byte loads of W rows), shuffle-reduce
 //   dgrad : dX[M,K] (+)= alpha * dZ W (* mask)      thread = 4 consecutive k (16-byte loads of W rows), N split over blockIdx.y,
 //                                                   partial sums (already masked / scaled: both are linear) added atomically
@@ -125,7 +125,7 @@ __global__ void __launch_bounds__(128) fewrows_dgrad_kernel(const float* __restr
       if (k + j >= K) continue;
       float v = alpha * acc[r][j];
       if (relu_src && !(relu_src[(size_t)(m0 + r) * ld_relu + k + j] > 0.f)) v = 0.f;      // mask and alpha are linear: applied per partial
-      if (v != 0.f) atomicAdd(dX + (size_t)(m0 + r) * lddx + k + j, v);
+      dX[((size_t)blockIdx.y * M + m0 + r) * lddx + k + j] = v;      // this contraction slice's partial ([slices][M][K]), summed in order
     }
   }
 }
@@ -474,12 +474,15 @@ int launch_fewrows_dgrad(const float* dZ, int lddz, const float* W, int ldw, con
     return ft_launch(fewrows_dgrad_tiled_kernel, dim3(tiles, S), S, FT_DG_SMEM, st, dZ, lddz, W, ldw, inv_sigma, relu_src, ld_relu, dX, lddx, M, N, K,
                      accumulate, n_per_cta);
   }
-  if (!accumulate) GCBF_CUDA_OK(cudaMemset2DAsync(dX, (size_t)lddx * 4, 0, (size_t)K * 4, M, st));
+  const int slices = ceil_div(N, FRD_NSLICE);
+  float* part = nullptr;
+  GCBF_CUDA_OK(scratch_alloc((void**)&part, (size_t)slices * M * K * 4, st));
   for (int m0 = 0; m0 < M; m0 += FR_MT) {
-    fewrows_dgrad_kernel<<<dim3(ceil_div(K, 512), ceil_div(N, FRD_NSLICE)), 128, 0, st>>>(dZ, lddz, W, ldw, inv_sigma, relu_src, ld_relu, dX, lddx, M,
-                                                                                       N, K, m0);
+    fewrows_dgrad_kernel<<<dim3(ceil_div(K, 512), slices), 128, 0, st>>>(dZ, lddz, W, ldw, inv_sigma, relu_src, ld_relu, part, K, M, N, K, m0);
     GCBF_LAUNCH_OK();
   }
+  GCBF_CUDA_OK(add_partials(part, slices, M, K, dX, lddx, accumulate, st));
+  GCBF_CUDA_OK(scratch_free(part, st));
   return GCBF_OK;
 }
 

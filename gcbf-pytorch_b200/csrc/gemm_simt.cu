@@ -1,5 +1,5 @@
 // fp32 SIMT GEMM with fused epilogues -- the exact-fp32 implementation of the linear layers of gcbf.nn.MLP
-// (reference gcbf/nn/mlp.py:44-47).  Used for every shape the tcgen05 path does not take (odd K such as
+// (reference gcbf/nn/mlp.py:44-47).  Used for every shape the wgmma path does not take (odd K such as
 // the 12..14-wide first phi layer, the tiny gate / head layers) and as the numerical cross-check of the
 // tensor-core kernel.  One kernel, three operand layouts:
 //
@@ -27,7 +27,7 @@ struct Epi {
   const float* relu_src;  // [M, ld_relu] or nullptr   (DGRAD)
   int ld_relu;
   int accumulate;         // WGRAD / DGRAD: add into C
-  int atomic;             // WGRAD: split-K partials via atomicAdd
+  size_t split_stride;    // WGRAD split-K: contraction split z writes the slice C + z * split_stride
 };
 
 // Load one BK x 128 operand tile into registers (8 floats per thread).
@@ -170,12 +170,8 @@ __global__ void __launch_bounds__(NT) gemm_simt_kernel(const float* __restrict__
             if (j < nv) v[j] = (__ldg(ep.relu_src + (size_t)m * ep.ld_relu + n + j) > 0.f) ? v[j] : 0.f;
         }
       }
-      float* dst = C + (size_t)m * ldc + n;
-      if (ep.mode == EPI_WGRAD && ep.atomic) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (j < nv) atomicAdd(dst + j, v[j]);
-      } else if (ep.accumulate) {
+      float* dst = C + (size_t)blockIdx.z * ep.split_stride + (size_t)m * ldc + n;
+      if (ep.accumulate) {
 #pragma unroll
         for (int j = 0; j < 4; ++j)
           if (j < nv) dst[j] += v[j];
@@ -206,7 +202,7 @@ __global__ void colsum_kernel(const float* __restrict__ dZ, int ld, int M, int N
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += part[i][threadIdx.x];
-    if (gridDim.y > 1) atomicAdd(db + col, t);
+    if (gridDim.y > 1) db[(size_t)blockIdx.y * N + col] = t;     // row block's partial; summed in order by add_partials
     else if (accumulate) db[col] += t;
     else db[col] = t;
   }
@@ -230,10 +226,18 @@ int launch_colsum(const float* dZ, int ld, int M, int N, float* db, int accumula
   int rsplit = (int)imin64(64, imax64(1, (int64_t)M / 2048));
   int rows_per_block = ceil_div(M, rsplit);
   rsplit = ceil_div(M, rows_per_block);
-  if (rsplit > 1 && !accumulate) GCBF_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)N * 4, st));
   dim3 g2(ceil_div(N, 32), rsplit), b2(32, 8);
-  colsum_kernel<<<g2, b2, 0, st>>>(dZ, ld, M, N, db, accumulate, rows_per_block);
+  if (rsplit == 1) {
+    colsum_kernel<<<g2, b2, 0, st>>>(dZ, ld, M, N, db, accumulate, rows_per_block);
+    GCBF_LAUNCH_OK();
+    return GCBF_OK;
+  }
+  float* part = nullptr;
+  GCBF_CUDA_OK(scratch_alloc((void**)&part, (size_t)rsplit * N * 4, st));
+  colsum_kernel<<<g2, b2, 0, st>>>(dZ, ld, M, N, part, accumulate, rows_per_block);
   GCBF_LAUNCH_OK();
+  GCBF_CUDA_OK(add_partials(part, rsplit, 1, N, db, N, accumulate, st));
+  GCBF_CUDA_OK(scratch_free(part, st));
   return GCBF_OK;
 }
 
@@ -268,11 +272,22 @@ int launch_simt_wgrad(const float* dZ, int lddz, const float* X, int ldx, const 
   int k_chunk = ceil_div(ceil_div(M, splits), BK) * BK;
   splits = ceil_div(M, k_chunk);
   Epi ep{};
-  ep.mode = EPI_WGRAD; ep.alpha = inv_sigma; ep.accumulate = accumulate; ep.atomic = splits > 1;
-  if (splits > 1 && !accumulate) GCBF_CUDA_OK(cudaMemset2DAsync(dW, (size_t)lddw * 4, 0, (size_t)K * 4, N, st));
+  ep.mode = EPI_WGRAD; ep.alpha = inv_sigma; ep.accumulate = accumulate;
   dim3 grid(ceil_div(K, BN), ceil_div(N, BM), splits);
-  gemm_simt_kernel<false, false><<<grid, NT, 0, st>>>(dZ, lddz, X, ldx, dW, lddw, N, K, M, k_chunk, ep);
-  GCBF_LAUNCH_OK();
+  if (splits == 1) {
+    gemm_simt_kernel<false, false><<<grid, NT, 0, st>>>(dZ, lddz, X, ldx, dW, lddw, N, K, M, k_chunk, ep);
+    GCBF_LAUNCH_OK();
+  } else {
+    // each contraction split writes its own [N][K] slice; the slices are summed in order
+    float* part = nullptr;
+    GCBF_CUDA_OK(scratch_alloc((void**)&part, (size_t)splits * N * K * 4, st));
+    ep.accumulate = 0;
+    ep.split_stride = (size_t)N * K;
+    gemm_simt_kernel<false, false><<<grid, NT, 0, st>>>(dZ, lddz, X, ldx, part, K, N, K, M, k_chunk, ep);
+    GCBF_LAUNCH_OK();
+    GCBF_CUDA_OK(add_partials(part, splits, N, K, dW, lddw, accumulate, st));
+    GCBF_CUDA_OK(scratch_free(part, st));
+  }
   if (db) return launch_colsum(dZ, lddz, M, N, db, accumulate, st);
   return GCBF_OK;
 }

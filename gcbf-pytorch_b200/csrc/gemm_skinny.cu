@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) skinny_fwd_kernel(const float* __restrict
 }
 
 // The same layer writing its output directly as a tile-scaled fp16 [hi|lo] companion (the format the tensor-core epilogues emit,
-// gemm_tcgen05_f16.cu): a block owns one 128-row x 256-column tile; with K <= 16 an output costs 2*K flops, so the tile is computed
+// gemm_wgmma_f16.cu): a block owns one 128-row x 256-column tile; with K <= 16 an output costs 2*K flops, so the tile is computed
 // TWICE -- once for its exact max|y| (the tile's scale), once to convert and store -- instead of writing fp32, re-reading it for an
 // amax pass and again for a split pass (12 B/element of HBM traffic become 4).
 __device__ __forceinline__ uint32_t skinny_scale_bits(uint32_t amax_bits) {     // == th::scale_bits_from_amax
@@ -359,10 +359,11 @@ __global__ void __launch_bounds__(256) skinny_wgrad_kernel(const float* __restri
   }
   if (n < N) {
     const float alpha = alpha_p ? __ldg(alpha_p) : 1.f;
+    // this row block's partials (dW_part [row block][N][K], db_part [row block][N]); summed in order by add_partials
 #pragma unroll
     for (int k = 0; k < SK; ++k)
-      if (k < K) atomicAdd(dW + (size_t)n * lddw + k, alpha * acc[k]);
-    if (db) atomicAdd(db + n, accb);
+      if (k < K) dW[((size_t)blockIdx.y * N + n) * K + k] = alpha * acc[k];
+    if (db) db[(size_t)blockIdx.y * N + n] = accb;
   }
 }
 
@@ -413,16 +414,18 @@ int launch_skinny_dgrad(const float* dZ, int lddz, const float* W, int ldw, cons
 
 int launch_skinny_wgrad(const float* dZ, int lddz, const float* X, int ldx, const float* inv_sigma, float* dW, int lddw,
                         float* db, int M, int N, int K, int accumulate, cudaStream_t st) {
-  if (!accumulate) {
-    GCBF_CUDA_OK(cudaMemset2DAsync(dW, (size_t)lddw * 4, 0, (size_t)K * 4, N, st));
-    if (db) GCBF_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)N * 4, st));
-  }
   const int col_blocks = ceil_div(N, 256);
   int row_blocks = max(1, min(ceil_div(M, 4 * SK_ROWS), (4 * kNumSMs) / col_blocks));
   const int rpb = ceil_div(ceil_div(M, row_blocks), SK_ROWS) * SK_ROWS;
   row_blocks = ceil_div(M, rpb);
-  skinny_wgrad_kernel<<<dim3(col_blocks, row_blocks), 256, 0, st>>>(dZ, lddz, X, ldx, inv_sigma, dW, lddw, db, M, N, K, rpb);
+  float* part = nullptr;
+  GCBF_CUDA_OK(scratch_alloc((void**)&part, (size_t)row_blocks * N * (K + 1) * 4, st));
+  float* db_part = part + (size_t)row_blocks * N * K;
+  skinny_wgrad_kernel<<<dim3(col_blocks, row_blocks), 256, 0, st>>>(dZ, lddz, X, ldx, inv_sigma, part, lddw, db ? db_part : nullptr, M, N, K, rpb);
   GCBF_LAUNCH_OK();
+  GCBF_CUDA_OK(add_partials(part, row_blocks, N, K, dW, lddw, accumulate, st));
+  if (db) GCBF_CUDA_OK(add_partials(db_part, row_blocks, 1, N, db, N, accumulate, st));
+  GCBF_CUDA_OK(scratch_free(part, st));
   return GCBF_OK;
 }
 

@@ -120,15 +120,18 @@ __global__ void __launch_bounds__(256) colsum_narrow_kernel(const float* __restr
     float t = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) t += part[w][threadIdx.x];
-    atomicAdd(db + threadIdx.x, t);
+    db[(size_t)blockIdx.x * N + threadIdx.x] = t;      // this block's partial; summed in order by add_partials
   }
 }
 
 int launch_colsum_narrow(const float* dZ, int ld, int M, int N, float* db, int accumulate, cudaStream_t st) {
-  if (!accumulate) GCBF_CUDA_OK(cudaMemsetAsync(db, 0, (size_t)N * 4, st));
   const int blocks = (int)imax64(1, imin64(ceil_div(M, 256), 2 * kNumSMs));
-  colsum_narrow_kernel<<<blocks, 256, 0, st>>>(dZ, ld, M, N, db);
+  float* part = nullptr;
+  GCBF_CUDA_OK(scratch_alloc((void**)&part, (size_t)blocks * N * 4, st));
+  colsum_narrow_kernel<<<blocks, 256, 0, st>>>(dZ, ld, M, N, part);
   GCBF_LAUNCH_OK();
+  GCBF_CUDA_OK(add_partials(part, blocks, 1, N, db, N, accumulate, st));
+  GCBF_CUDA_OK(scratch_free(part, st));
   return GCBF_OK;
 }
 

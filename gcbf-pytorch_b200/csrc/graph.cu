@@ -270,6 +270,112 @@ extern "C" int gcbf_edge_attr_fwd(int env, const float* states, int ld_state, co
   return GCBF_OK;
 }
 
+namespace gcbf {
+
+// Deterministic form of the same scatter for callers that know the node count: every edge writes its two contributions to
+// scratch, then one thread per node adds them in edge order -- target side from the node's contiguous run of the (target-sorted)
+// edge list, source side from a counting sort of the edges by source -- so d_states does not depend on the order edges run in.
+template <int ENV, int SD, int ED>
+__global__ void edge_attr_contrib_kernel(const float* __restrict__ states, int ld, const int64_t* __restrict__ ei, int64_t E,
+                                         const float* __restrict__ d_e, float* __restrict__ contrib, int32_t* __restrict__ src_count) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const int64_t node[2] = {ei[e], ei[E + e]};
+  float g[ED];
+#pragma unroll
+  for (int k = 0; k < ED; ++k) g[k] = d_e[e * ED + k];
+#pragma unroll
+  for (int side = 0; side < 2; ++side) {
+    const float sgn = side == 0 ? 1.f : -1.f;
+    float ds[SD];
+    if (ENV == GCBF_ENV_DUBINS_CAR) {
+      const float th = __ldg(states + node[side] * ld + 2), v = __ldg(states + node[side] * ld + 3);
+      const float c = cosf(th), s = sinf(th);
+      ds[0] = g[0]; ds[1] = g[1];
+      ds[2] = g[2] + g[3] * (-v * s) + g[4] * (v * c);
+      ds[3] = g[3] * c + g[4] * s;
+    } else {
+#pragma unroll
+      for (int k = 0; k < SD; ++k) ds[k] = g[k];
+    }
+#pragma unroll
+    for (int k = 0; k < SD; ++k) contrib[(side * E + e) * SD + k] = sgn * ds[k];
+  }
+  atomicAdd(src_count + node[0], 1);
+}
+
+__global__ void edge_src_fill_kernel(const int64_t* __restrict__ ei, int64_t E, int32_t* __restrict__ cursor, int32_t* __restrict__ ids) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < E) ids[atomicAdd(cursor + ei[e], 1)] = (int32_t)e;
+}
+
+template <int SD>
+__global__ void edge_attr_gather_kernel(const int64_t* __restrict__ ei, int64_t E, int num_nodes, const float* __restrict__ contrib,
+                                        const int32_t* __restrict__ src_off, int32_t* __restrict__ ids, float* __restrict__ d_states, int ld) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= num_nodes) return;
+  float acc[SD];
+#pragma unroll
+  for (int k = 0; k < SD; ++k) acc[k] = 0.f;
+  // source side: this node's edges in ascending edge order (the fill order above is arbitrary)
+  const int b = src_off[n], t = src_off[n + 1];
+  for (int i = b + 1; i < t; ++i) {
+    const int32_t v = ids[i];
+    int j = i - 1;
+    while (j >= b && ids[j] > v) { ids[j + 1] = ids[j]; --j; }
+    ids[j + 1] = v;
+  }
+  for (int i = b; i < t; ++i)
+#pragma unroll
+    for (int k = 0; k < SD; ++k) acc[k] += contrib[(int64_t)ids[i] * SD + k];
+  // target side: the contiguous run of edges whose target is n
+  const int64_t* dst = ei + E;
+  int64_t lo = 0, hi = E;
+  while (lo < hi) { const int64_t mid = (lo + hi) >> 1; if (dst[mid] < n) lo = mid + 1; else hi = mid; }
+  for (int64_t e = lo; e < E && dst[e] == n; ++e)
+#pragma unroll
+    for (int k = 0; k < SD; ++k) acc[k] += contrib[(E + e) * SD + k];
+#pragma unroll
+  for (int k = 0; k < SD; ++k) d_states[(int64_t)n * ld + k] += acc[k];
+}
+
+template <int ENV, int SD, int ED>
+static int edge_attr_bwd_ordered_t(const float* states, int ld, const int64_t* ei, int64_t E, int num_nodes, const float* d_e,
+                                   float* d_states, cudaStream_t st) {
+  // scratch: contributions [2][E][SD] floats, source offsets [N + 1], fill cursors [N], edge ids [E]
+  const size_t cbytes = (size_t)2 * E * SD * 4, obytes = ((size_t)num_nodes + 1) * 4;
+  uint8_t* buf = nullptr;
+  GCBF_CUDA_OK(scratch_alloc((void**)&buf, cbytes + 2 * obytes + (size_t)E * 4, st));
+  float* contrib = reinterpret_cast<float*>(buf);
+  int32_t* off = reinterpret_cast<int32_t*>(buf + cbytes);
+  int32_t* cursor = reinterpret_cast<int32_t*>(buf + cbytes + obytes);
+  int32_t* ids = reinterpret_cast<int32_t*>(buf + cbytes + 2 * obytes);
+  GCBF_CUDA_OK(cudaMemsetAsync(off, 0, obytes, st));
+  edge_attr_contrib_kernel<ENV, SD, ED><<<ceil_div(E, 256), 256, 0, st>>>(states, ld, ei, E, d_e, contrib, off);
+  GCBF_LAUNCH_OK();
+  GCBF_CUDA_OK(exclusive_scan_i32(off, num_nodes, st));
+  GCBF_CUDA_OK(cudaMemcpyAsync(cursor, off, (size_t)num_nodes * 4, cudaMemcpyDeviceToDevice, st));
+  edge_src_fill_kernel<<<ceil_div(E, 256), 256, 0, st>>>(ei, E, cursor, ids);
+  GCBF_LAUNCH_OK();
+  edge_attr_gather_kernel<SD><<<ceil_div(num_nodes, 128), 128, 0, st>>>(ei, E, num_nodes, contrib, off, ids, d_states, ld);
+  GCBF_LAUNCH_OK();
+  GCBF_CUDA_OK(scratch_free(buf, st));
+  return GCBF_OK;
+}
+
+int edge_attr_bwd_ordered(int env, const float* states, int ld_state, const int64_t* edge_index, int64_t num_edges, int num_nodes,
+                          const float* d_edge_attr, float* d_states, cudaStream_t st) {
+  if (num_edges == 0) return GCBF_OK;
+  switch (env) {
+    case GCBF_ENV_SIMPLE_CAR: return edge_attr_bwd_ordered_t<GCBF_ENV_SIMPLE_CAR, 4, 4>(states, ld_state, edge_index, num_edges, num_nodes, d_edge_attr, d_states, st);
+    case GCBF_ENV_DUBINS_CAR: return edge_attr_bwd_ordered_t<GCBF_ENV_DUBINS_CAR, 4, 5>(states, ld_state, edge_index, num_edges, num_nodes, d_edge_attr, d_states, st);
+    case GCBF_ENV_SIMPLE_DRONE: return edge_attr_bwd_ordered_t<GCBF_ENV_SIMPLE_DRONE, 6, 6>(states, ld_state, edge_index, num_edges, num_nodes, d_edge_attr, d_states, st);
+    default: set_error("edge_attr_bwd_ordered: unknown env %d", env); return GCBF_E_INVALID;
+  }
+}
+
+}  // namespace gcbf
+
 extern "C" int gcbf_edge_attr_bwd(int env, const float* states, int ld_state, const int64_t* edge_index,
                                   int64_t num_edges, const float* d_edge_attr, float* d_states, void* stream) {
   GCBF_REQUIRE(states && d_states && (num_edges == 0 || (edge_index && d_edge_attr)), "gcbf_edge_attr_bwd: null pointer");

@@ -1,5 +1,5 @@
 // C-ABI dispatch of the fp32 linear layers (K3): skinny-K stream kernels for in-features <= 16, otherwise the exact-fp32
-// SIMT tile kernel.  (Big layers run on the tensor cores through gcbf_linear_*_h, gemm_tcgen05_f16.cu.)  Reference op site: gcbf/nn/mlp.py:44-47 (nn.Linear + ReLU chain).
+// SIMT tile kernel.  (Big layers run on the tensor cores through gcbf_linear_*_h, gemm_wgmma_f16.cu.)  Reference op site: gcbf/nn/mlp.py:44-47 (nn.Linear + ReLU chain).
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -43,8 +43,8 @@ using namespace gcbf;
 static thread_local int g_last_impl = 0;
 extern "C" int gcbf_last_gemm_impl(void) { return g_last_impl; }
 
-extern "C" int gcbf_has_tcgen05(void) {
-#ifdef GCBF_WITH_TCGEN05
+extern "C" int gcbf_has_wgmma(void) {
+#ifdef GCBF_WITH_WGMMA
   return 1;
 #else
   return 0;
@@ -62,7 +62,7 @@ extern "C" int gcbf_linear_fwd(const float* X, int ldx, const float* W, int ldw,
   if (out_amax) GCBF_CUDA_OK(cudaMemsetAsync(out_amax, 0, 4, st));
   if (M == 0) return GCBF_OK;
   GCBF_REQUIRE(X && W && Y, "gcbf_linear_fwd: null pointer");
-  if (impl == 2) { set_error("gcbf_linear_fwd: the tcgen05 path has its own entry point (gcbf_linear_fwd_h)"); return GCBF_E_UNSUPPORTED; }
+  if (impl == 2) { set_error("gcbf_linear_fwd: the wgmma path has its own entry point (gcbf_linear_fwd_h)"); return GCBF_E_UNSUPPORTED; }
   if (impl == 0 && skinny_supported(K) && N >= 64 && M >= 64) {   // K <= 16: HBM-bound stream, not a GEMM tile
     g_last_impl = 3;
     return launch_skinny_fwd(X, ldx, W, ldw, bias, inv_sigma, Y, ldy, M, N, K, act, reinterpret_cast<uint32_t*>(out_amax), st);
@@ -90,7 +90,7 @@ extern "C" int gcbf_linear_bwd_data(const float* dZ, int lddz, const float* W, i
   if (M == 0) return GCBF_OK;
   GCBF_REQUIRE(dZ && W && dX, "gcbf_linear_bwd_data: null pointer");
   cudaStream_t st = as_stream(stream);
-  if (impl == 2) { set_error("gcbf_linear_bwd_data: the tcgen05 path has its own entry point (gcbf_linear_bwd_data_h)"); return GCBF_E_UNSUPPORTED; }
+  if (impl == 2) { set_error("gcbf_linear_bwd_data: the wgmma path has its own entry point (gcbf_linear_bwd_data_h)"); return GCBF_E_UNSUPPORTED; }
   if (impl == 0 && skinny_supported(K) && N >= 64 && M >= 64) {
     g_last_impl = 3;
     return launch_skinny_dgrad(dZ, lddz, W, ldw, inv_sigma, relu_src, ld_relu, dX, lddx, M, N, K, accumulate, st);
@@ -125,7 +125,7 @@ extern "C" int gcbf_linear_bwd_weight(const float* dZ, int lddz, const float* X,
     return GCBF_OK;
   }
   GCBF_REQUIRE(dZ && X, "gcbf_linear_bwd_weight: null pointer");
-  if (impl == 2) { set_error("gcbf_linear_bwd_weight: the tcgen05 path has its own entry point (gcbf_linear_bwd_weight_h)"); return GCBF_E_UNSUPPORTED; }
+  if (impl == 2) { set_error("gcbf_linear_bwd_weight: the wgmma path has its own entry point (gcbf_linear_bwd_weight_h)"); return GCBF_E_UNSUPPORTED; }
   if (impl == 0 && skinny_supported(K) && N >= 64 && M >= 64) {
     g_last_impl = 3;
     return launch_skinny_wgrad(dZ, lddz, X, ldx, inv_sigma, dW, lddw, db, M, N, K, accumulate, st);

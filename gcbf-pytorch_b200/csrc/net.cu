@@ -6,7 +6,7 @@
 //   gcbf/controller/gnn_controller.py:29-48   GNNController.forward: layer -> x[agent_mask] -> feat_2_action(cat[x, u_ref])
 // and their autograd backward.  Nothing here allocates device memory: every activation, fp16 companion, amax word and scratch
 // gradient is a bump allocation out of the caller's workspace; the *_workspace_bytes queries replay the same allocation sequence
-// without launching.  Per layer the dispatch rule is: tensor cores (3xFP16 tcgen05 kernel, gemm_tcgen05_f16.cu) when
+// without launching.  Per layer the dispatch rule is: tensor cores (3xFP16 wgmma kernel, gemm_wgmma_f16.cu) when
 // gcbf_linear_h_supported(M, N, K), else the fp32 kernels behind gcbf_linear_* (skinny-K / row-streaming / SIMT tile).
 #include <atomic>
 #include <vector>
@@ -119,7 +119,7 @@ int sn_power_iter(Run& R, const gcbf_linear_desc* const* layers, int n, bool sna
 }
 
 // ---- MLP chain -------------------------------------------------------------------------------------------------------
-// Companions written by the producing GEMM's epilogue ("emission", gemm_tcgen05_f16.cu): when a tensor-core layer's output (forward)
+// Companions written by the producing GEMM's epilogue ("emission", gemm_wgmma_f16.cu): when a tensor-core layer's output (forward)
 // or input gradient (backward) feeds another tensor-core layer, the producer writes it directly as a tile-scaled fp16 [hi|lo]
 // companion -- no amax pass, no split pass, no fp32 copy in HBM; the ReLU mask of the backward is read from the hi plane and the
 // bias gradient (column sums of dZ) is accumulated by the producing data-grad epilogue.  GCBF_EPI_H=0 keeps the split kernels.

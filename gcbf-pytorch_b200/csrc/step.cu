@@ -190,7 +190,7 @@ static int step_backward(Run& R, const gcbf_step_desc& d, const gcbf_step_batch&
   if (!R.dry) {
     // edge_attr(x+) -> x+ -> clamp(u + u_ref) -> actions  (VJP of forward_graph, gcbf.py:193)
     CHAIN_CUDA(cudaMemsetAsync(d_states, 0, (size_t)Nn * s * 4, main));
-    CHAIN_CALL(gcbf_edge_attr_bwd(d.env.env, c->states_next, s, b.edge_index, E, d_ea, d_states, main));
+    CHAIN_CALL(edge_attr_bwd_ordered(d.env.env, c->states_next, s, b.edge_index, E, Nn, d_ea, d_states, main));
     CHAIN_CALL(gcbf_step_bwd(&cfg, d_states, s, c->pass_mask, d_act_dyn, main));
     R.launched(E ? 2 : 1);
   }

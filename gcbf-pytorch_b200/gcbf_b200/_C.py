@@ -38,7 +38,7 @@ _SIGS = {
     'gcbf_abi_version': (c_int, []),
     'gcbf_abi_struct_size': (c_size_t, [c_int]),
     'gcbf_launch_count': (c_longlong, [c_int]),
-    'gcbf_has_tcgen05': (c_int, []),
+    'gcbf_has_wgmma': (c_int, []),
     'gcbf_last_gemm_impl': (c_int, []),
     'gcbf_radius_graph_count': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, P, P]),
     'gcbf_radius_graph_fill': (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, P, P, c_int64, P]),
@@ -191,4 +191,4 @@ def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError('gcbf_b200 ops need CUDA tensors: there is no CPU fallback '
-                               '(build container has no GPU; run under gpurun)')
+                               '(build the library with __graft_entry__.build() and run on a GPU)')

@@ -1,4 +1,4 @@
-"""gcbf_b200 -- B200-native (sm_100a) implementation of the gcbf-pytorch hot path.
+"""gcbf_b200 -- H100-native (sm_90a) implementation of the gcbf-pytorch hot path.
 
 Mirrors the reference package layout (`gcbf.nn`, `gcbf.controller`, `gcbf.algo`, `gcbf.env`) with the same class
 names, constructor signatures, forward signatures and state-dict keys; the arithmetic runs in the hand-written

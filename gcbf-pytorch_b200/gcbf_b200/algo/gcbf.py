@@ -1,4 +1,4 @@
-"""GCBF: CBF network + actor + the train step of reference gcbf/algo/gcbf.py:64-309 on the sm_100a kernels.
+"""GCBF: CBF network + actor + the train step of reference gcbf/algo/gcbf.py:64-309 on the sm_90a kernels.
 
 What changes relative to the reference's `update` body (results identical, see tests/test_parity_gpu.py):
   * safe/unsafe masks and the re-linked radius graphs are ONE kernel launch over the whole batch instead of

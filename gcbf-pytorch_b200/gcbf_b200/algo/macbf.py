@@ -1,4 +1,4 @@
-"""MACBF, the paper's baseline algorithm (reference gcbf/algo/macbf.py:20-239; SURVEY 8f-4), on the sm_100a kernels.
+"""MACBF, the paper's baseline algorithm (reference gcbf/algo/macbf.py:20-239; SURVEY 8f-4), on the sm_90a kernels.
 
 Differences from GCBF that matter for the kernels: the CBF is a per-EDGE value h_ij (an MLP on cat[x_i, x_j, e_ij], no aggregation),
 the actor aggregates with a per-target MAX, the safe / unsafe sets are per-edge distance tests, the h_dot condition uses the

@@ -3,7 +3,7 @@ chunks.
 
 Why: one train step allocates ~10 GB of short-lived tensors whose sizes change every step (the re-linked graph has a
 different edge count each time), which makes the torch caching allocator fall back to cudaMalloc / cudaFree storms
-(measured: the same step taking 31 ms or 70 ms).  With 180 GB of HBM per GPU the simple answer is an explicit arena:
+(measured: the same step taking 31 ms or 70 ms).  With 80 GB of HBM per GPU the simple answer is an explicit arena:
 `begin()` at the start of `GCBF.train_step`, every internal buffer is a view into a chunk, nothing is freed, the next
 `begin()` rewinds.  Tensors handed back to the caller are cloned out of the arena first.
 """

@@ -2,7 +2,7 @@
 rows, concatenated with the nominal control u_ref and reduced by a 4-layer head to the action correction.  Same constructor,
 sub-module names (= checkpoint keys `feat_transformer.module_0.*`, `feat_2_action.net.*`) and `forward(data)` contract as the
 reference's gcbf/controller/gnn_controller.py:13-48; here the whole chain -- edge MLP, aggregation, node MLP, row selection,
-concat, head -- is ONE autograd node over the sm_100a kernels (`ops.GNNNetFunction`, reached through the layer's `run`)."""
+concat, head -- is ONE autograd node over the sm_90a kernels (`ops.GNNNetFunction`, reached through the layer's `run`)."""
 from torch import Tensor
 
 from ..data import agent_row_index

@@ -1,6 +1,6 @@
 """MultiAgentEnv: the reference's environment interface (gcbf/env/base.py:11-398) with the hot-path methods
 -- radius graph, edge features, nominal controller, finite-difference step, safe/unsafe masks -- running in
-the sm_100a kernels, batched over all graphs of a `Batch` in ONE launch instead of the reference's per-graph
+the sm_90a kernels, batched over all graphs of a `Batch` in ONE launch instead of the reference's per-graph
 Python loops (`to_data_list()` at simple_car.py:313, 338 and the re-linking loop at gcbf/algo/gcbf.py:195-199).
 
 Graph layout contract (what every reference env produces): per graph the `num_agents` agents come first, then the

@@ -1,4 +1,4 @@
-"""CBFGNNLayer / ControllerGNNLayer (reference gcbf/nn/gnn.py:14-79) on the sm_100a kernels.
+"""CBFGNNLayer / ControllerGNNLayer (reference gcbf/nn/gnn.py:14-79) on the sm_90a kernels.
 
 One message-passing layer:  m_ij = phi(cat[x_i, x_j, e_ij]);  a = softmax_i(gate_nn(m));  aggr_i = sum_j a_ij m_ij;
 out_i = gamma(cat[aggr_i, x_i]).  Signature, attribute names (`phi`, `gamma`, `aggr_module.gate_nn`) and

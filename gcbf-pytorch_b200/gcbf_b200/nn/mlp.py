@@ -1,4 +1,4 @@
-"""gcbf.nn.MLP on the sm_100a kernels.
+"""gcbf.nn.MLP on the sm_90a kernels.
 
 Same constructor, same `.net` nn.Sequential (so the state-dict keys `net.{0,2,4}.{weight|weight_orig,weight_u,
 weight_v,bias}` and the RNG stream of the initialisation are identical to reference gcbf/nn/mlp.py:9-47), but

@@ -1,4 +1,4 @@
-"""Host-side orchestration of the sm_100a kernels: raw op wrappers (one C-ABI call each) and the two
+"""Host-side orchestration of the sm_90a kernels: raw op wrappers (one C-ABI call each) and the two
 autograd.Functions the nn.Modules are built from.
 
     GNNNetFunction   edge-MLP phi -> attention aggregation -> node-MLP gamma [-> row select -> head MLP]
@@ -26,7 +26,7 @@ ACT_NONE, ACT_RELU, ACT_TANH = 0, 1, 2
 # entry points of the library (csrc/net.cu, csrc/step.cu): same kernels, same order -- an A/B switch for debugging only.
 NATIVE = os.environ.get('GCBF_NATIVE', '1') != '0'
 ENV_IDS = {'SimpleCar': 0, 'DubinsCar': 1, 'SimpleDrone': 2}
-GEMM_IMPL = 0   # 0 auto, 1 force fp32 SIMT, 2 force tcgen05 (tests flip this)
+GEMM_IMPL = 0   # 0 auto, 1 force fp32 SIMT, 2 force wgmma (tests flip this)
 
 
 class _GemmTimer:
@@ -110,7 +110,7 @@ class _GemmTimer:
         if shapes:
             tag, (tms, tfl, tn) = max(shapes.items(), key=lambda kv: kv[1][0])
             dominant = dict(product=tag[0], M=tag[1], N=tag[2], K=tag[3], launches=tn, ms_per_launch=tms / tn, flops_per_launch=tfl / tn)
-        return dict(kernel='gemm_tcgen05_3xfp16' if tensor else 'gemm_simt_kernel', ms=ms, flops=flops, launches=n, tensor=tensor,
+        return dict(kernel='gemm_wgmma_3xfp16' if tensor else 'gemm_simt_kernel', ms=ms, flops=flops, launches=n, tensor=tensor,
                     prep_ms=prep_ms, prep_launches=nprep, dominant=dominant,
                     other_ms=(by[1] if tensor else by[2])[0], other_flops=(by[1] if tensor else by[2])[1])
 
@@ -135,7 +135,7 @@ def _mat(t: torch.Tensor) -> Tuple[torch.Tensor, int]:
 # ----------------------------------------------------------------------------------------------------
 # raw ops (each = one C-ABI entry point)
 # ----------------------------------------------------------------------------------------------------
-USE_TCGEN05 = True     # set False to keep every layer on the fp32 SIMT kernel
+USE_WGMMA = True     # set False to keep every layer on the fp32 SIMT kernel
 WEIGHT_EPOCH = 0       # bumped whenever a raw kernel rewrites parameters (GCBF.optim_step): invalidates weight companions
 
 
@@ -143,7 +143,7 @@ WEIGHT_EPOCH = 0       # bumped whenever a raw kernel rewrites parameters (GCBF.
 class H16:
     """fp16 [hi | lo] companion of an fp32 matrix (same row-major layout, pitch `ld` halves): x * s = hi + lo with the
     per-tensor power-of-two scale s derived from `amax` (device int32 = float bits of max|x|).  One companion serves
-    every GEMM the matrix takes part in (K-major or MN-major operand, csrc/gemm_tcgen05_f16.cu)."""
+    every GEMM the matrix takes part in (K-major or MN-major operand, csrc/gemm_wgmma_f16.cu)."""
     buf: torch.Tensor
     amax: torch.Tensor
     rows: int
@@ -152,8 +152,8 @@ class H16:
 
 
 def use_h(M: int, N: int, K: int) -> bool:
-    """Does the [M,K] x [N,K] layer (forward, data-grad and weight-grad alike) run on the tcgen05 3xFP16 kernel?"""
-    if not USE_TCGEN05 or GEMM_IMPL == 1:
+    """Does the [M,K] x [N,K] layer (forward, data-grad and weight-grad alike) run on the wgmma 3xFP16 kernel?"""
+    if not USE_WGMMA or GEMM_IMPL == 1:
         return False
     if GEMM_IMPL == 2:
         return True
@@ -676,7 +676,7 @@ class MLPCtx:
     acts: List[torch.Tensor] = field(default_factory=list)      # acts[0] = input, acts[l] = output of layer l
     inv_sigma: List[Optional[torch.Tensor]] = field(default_factory=list)
     uv: List[Optional[Tuple[torch.Tensor, torch.Tensor]]] = field(default_factory=list)
-    acts_h: List[Optional[H16]] = field(default_factory=list)  # acts_h[l] = fp16 companion of acts[l] when layer l is on tcgen05
+    acts_h: List[Optional[H16]] = field(default_factory=list)  # acts_h[l] = fp16 companion of acts[l] when layer l is on the wgmma kernel
     out_amax: Optional[torch.Tensor] = None                   # amax slot of the MLP's output when the caller asked for it
 
 
@@ -993,7 +993,7 @@ def net_backward(spec: NetSpec, ctx, d_out, rowptr, row_index, need_d_edge_attr)
 
 def sync_gemm_impl():
     """Tell the library which linear-layer implementation the chain-level calls may use (tests flip ops.GEMM_IMPL)."""
-    native.fn('gcbf_set_gemm_impl')(1 if (not USE_TCGEN05 or GEMM_IMPL == 1) else (2 if GEMM_IMPL == 2 else 0))
+    native.fn('gcbf_set_gemm_impl')(1 if (not USE_WGMMA or GEMM_IMPL == 1) else (2 if GEMM_IMPL == 2 else 0))
 
 
 def _grad_views(specs, device):

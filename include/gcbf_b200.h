@@ -1,5 +1,5 @@
 /*
- * gcbf_b200.h -- C ABI of libgcbf_b200.so: the B200 (sm_100a) hot path of MIT-REALM/gcbf-pytorch.
+ * gcbf_b200.h -- C ABI of libgcbf_b200.so: the H100 (sm_90a) hot path of MIT-REALM/gcbf-pytorch.
  *
  * The reference has no FFI of its own (it is pure Python on torch / torch_geometric); the boundary a
  * maintainer binds is therefore the set of tensor operations its Python classes perform.  Every entry
@@ -9,8 +9,12 @@
  *   - plain pointers and sizes only; all pointers are DEVICE pointers unless the name ends in `_host`;
  *   - all matrices are dense row-major fp32 with an explicit leading dimension (`ld*`, in elements);
  *     edge_index is int64 [2, E] (row 0 = source j, row 1 = target i), masks are uint8;
- *   - nothing here allocates or synchronises: outputs / workspaces are caller-provided, every launch
- *     goes to `stream` (a cudaStream_t passed as void*);
+ *   - nothing here synchronises, and outputs / workspaces are caller-provided; every launch goes to `stream` (a cudaStream_t
+ *     passed as void*).  Reductions over many blocks (split-K weight gradients, column sums, the train step's edge-feature VJP)
+ *     write per-block partials to short-lived scratch taken from the library's own stream-ordered memory pool (cudaMallocAsync
+ *     semantics, freed on `stream`, cached in the pool) and sum them in a fixed order, so results are run-to-run reproducible.
+ *     That scratch (up to a few tens of MB at the largest configurations) is NOT counted by the *_workspace_bytes queries;
+ *     an allocation failure is reported as GCBF_E_CUDA;
  *   - return value: 0 on success, negative GCBF_E_* on failure; gcbf_last_error() gives the text;
  *   - per-kernel entry points are thread-compatible (no global mutable state except the per-thread last-error string); the
  *     chain-level entry points of ABI v3 keep per-process state (seven CUDA events and one pinned word per device for the train
@@ -48,11 +52,11 @@ int gcbf_abi_version(void);
  * 3 gcbf_step_desc, 4 gcbf_step_batch, 5 gcbf_step_out, 6 gcbf_net_ctx, 7 gcbf_mlp_ctx, 8 gcbf_step_ctx, 9 gcbf_time_rec,
  * 10 gcbf_sn_layer, 11 gcbf_split_desc, 12 gcbf_h16; 0 for unknown): bindings check their mirrors against it */
 size_t gcbf_abi_struct_size(int which);
-/* 1 if the library was built with the tcgen05 (3xFP16) GEMM path compiled in, else 0 */
-int gcbf_has_tcgen05(void);
+/* 1 if the library was built with the wgmma (3xFP16) GEMM path compiled in, else 0 (ABI v5: was gcbf_has_tcgen05) */
+int gcbf_has_wgmma(void);
 /* which kernel the most recent gcbf_linear_* call on this thread launched: 1 = fp32 SIMT tile GEMM,
  * 3 = fp32 skinny-K stream kernel (in-features <= 16), 4 = row-streaming kernel (out-features <= 32), 5 = few-rows kernels
- * (M <= 64: rollout-time single-graph passes stream the weights instead of tiling the output).  (The tcgen05 path
+ * (M <= 64: rollout-time single-graph passes stream the weights instead of tiling the output).  (The wgmma path
  * has its own entry points, gcbf_linear_*_h.) */
 int gcbf_last_gemm_impl(void);
 
@@ -83,7 +87,8 @@ int gcbf_rowptr_from_targets(const int64_t* edge_dst, int64_t num_edges, int num
 /* ---------------------------------------------------------------------------------------------------
  * K2  edge features.  edge_attr = g(s[src]) - g(s[dst]); g = identity (SimpleCar, SimpleDrone:
  * simple_car.py:246-247, simple_drone.py:313-314) or [x,y,theta,v cos,v sin] (dubins_car.py:724-728).
- * bwd accumulates (atomicAdd) into d_states, which the caller zero-initialises.
+ * bwd accumulates (atomicAdd, so the summation order varies between runs) into d_states, which the caller zero-initialises;
+ * the chain-level train step and gcbf_apply use an ordered per-node sum instead.
  * edge_input builds cat([x_i, x_j, edge_attr]) (gnn.py:31, :68) into rows of leading dim ld_out,
  * zero-filling the columns past 2*node_dim+edge_dim.
  * ------------------------------------------------------------------------------------------------- */
@@ -115,7 +120,7 @@ int gcbf_linear_bwd_weight(const float* dZ, int lddz, const float* X, int ldx, c
                            float* dW, int lddw, float* db, int M, int N, int K, int accumulate, int impl,
                            void* stream);
 /* ---------------------------------------------------------------------------------------------------
- * K3 on the tensor cores (tcgen05 + TMEM + TMA, csrc/gemm_tcgen05_f16.cu): the same three products with
+ * K3 on the tensor cores (wgmma + TMA + mbarrier, csrc/gemm_wgmma_f16.cu): the same three products with
  * error-compensated 3xFP16 arithmetic (fp32-grade: 22 significand bits per operand, fp32 accumulation).
  * Operands are "companions": for an fp32 matrix X[rows, cols] the caller provides a device buffer of
  * 2*rows*ld_h halves (ld_h a multiple of 8, 16-byte aligned) that gcbf_split_f16 fills with the planes
@@ -156,7 +161,7 @@ int gcbf_linear_bwd_weight_h(const void* dZh, int lddzh, const void* dz_amax, co
  * scaled companion (Yh / dXh, output width > 128), because every CTA knows the exact maximum of its own 128 x 256 tile.  That
  * removes the amax + split passes (and the fp32 round trip through HBM) for every hidden activation / gradient between two
  * tensor-core layers.  Y / dX may be NULL when only the companion is wanted.  data-grad extras: the ReLU mask can be read from
- * the hi plane of the layer output's companion (relu_h; y > 0 <=> hi > 0), and `colsum` (optional) atomically accumulates the
+ * the hi plane of the layer output's companion (relu_h; y > 0 <=> hi > 0), and `colsum` (optional) accumulates (per-row-tile partials summed in a fixed order) the
  * column sums of the masked output (= the bias gradient of the layer below).  Weight companions stay per-tensor. */
 typedef struct gcbf_h16 {
   void* buf;                /* hi plane [rows][ld] halves, lo plane at buf + rows * ld halves */

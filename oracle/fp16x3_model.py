@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY -- CPU model of the arithmetic of the tensor-core linear layers (csrc/gemm_tcgen05_f16.cu).
+"""TEST INFRASTRUCTURE ONLY -- CPU model of the arithmetic of the tensor-core linear layers (csrc/gemm_wgmma_f16.cu).
 
 The product computes an fp32 GEMM as three fp16 tensor-core products of [hi | lo] companions.  This module restates that
 arithmetic in plain torch so that (a) the companion format is pinned bit-for-bit (tests/test_kernels_gpu.py compares the
@@ -10,7 +10,7 @@ import torch
 
 def scale_for(amax: torch.Tensor) -> float:
     """Power of two s with amax * s in [2^14, 2^15) (1 for zero / denormal / non-finite amax); mirrors
-    scale_bits_from_amax in csrc/gemm_tcgen05_f16.cu."""
+    scale_bits_from_amax in csrc/gemm_wgmma_f16.cu."""
     bits = amax.reshape(1).float().view(torch.int32).item()
     e = (bits >> 23) & 0xff
     if e in (0, 255):
@@ -50,7 +50,7 @@ TILE_ROWS, TILE_COLS = 128, 256
 
 def split_tiled(x: torch.Tensor):
     """Companion with one power-of-two scale per (128-row, 256-column) tile -- the format the producing GEMM's epilogue writes
-    (csrc/gemm_tcgen05_f16.cu, EPI emit): every output tile knows its own max|y| exactly, so no pass over the tensor and no
+    (csrc/gemm_wgmma_f16.cu, EPI emit): every output tile knows its own max|y| exactly, so no pass over the tensor and no
     a-priori bound is needed.  Returns (hi, lo, tile_amax [ceil(rows/128), ceil(cols/256)] float32).  Per tile the arithmetic is
     `split` above (scale_for(tile max), hi = fp16(x s), lo = fp16(x s - hi))."""
     rows, cols = x.shape

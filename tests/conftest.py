@@ -13,7 +13,7 @@ GOLDEN_DIR = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (pytest -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f'{name} declared in include/gcbf_b200.h but not exported'
     assert sorted(_C.EXPORTED_SYMBOLS) == declared, set(_C.EXPORTED_SYMBOLS) ^ set(declared)
-    assert _C.lib().gcbf_abi_version() == 4
+    assert _C.lib().gcbf_abi_version() == 5
 
 
 def test_env_cfg_struct_layout():
@@ -106,14 +106,27 @@ def test_state_dict_key_contract():
     assert act.state_dict()['feat_2_action.net.0.weight'].shape == (512, 1026)
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/pretrained'), reason='shipped checkpoints live in the reference checkout')
+def _checkpoint_like(env_name, out_dir):
+    """cbf.pkl / actor.pkl with the keys (in file order), shapes and per-tensor mean / std of the shipped checkpoint
+    pretrained/<env>/models/step_500000 (tests/golden/pretrained_stats.pt), written with torch.save like the reference's."""
+    stats = torch.load(os.path.join(ROOT, 'tests', 'golden', 'pretrained_stats.pt'), weights_only=False)[env_name]
+    g = torch.Generator().manual_seed(5)
+    os.makedirs(out_dir, exist_ok=True)
+    for net in ('cbf', 'actor'):
+        # the statistics record every tensor as a 2-D view: biases and the spectral-norm vectors u, v are 1-D in the files
+        sd = {k: torch.randn(st['shape'][1:] if k.endswith(('bias', 'weight_u', 'weight_v')) else st['shape'], generator=g) * st['std']
+              + st['mean'] for k, st in stats[net].items()}
+        torch.save(sd, os.path.join(out_dir, f'{net}.pkl'))
+    return out_dir
+
+
 @pytest.mark.parametrize('env_name', ['SimpleCar', 'DubinsCar', 'SimpleDrone'])
 def test_shipped_checkpoints_load_strictly(env_name, tmp_path):
-    """All six shipped checkpoint files (pretrained/<env>/models/step_500000/{cbf,actor}.pkl, SURVEY 8a row a13) load with
-    strict=True into the product modules through GCBF.load, also AFTER the parameters were re-homed into the flat bucket, and
-    GCBF.save writes files of the reference's size (no bucket-sized storages) that the oracle port reads back unchanged."""
+    """Checkpoint files laid out like the six shipped ones ({cbf,actor}.pkl with their keys and shapes, SURVEY 8a row a13) load
+    with strict=True into the product modules through GCBF.load, also AFTER the parameters were re-homed into the flat bucket,
+    and GCBF.save writes files of the checkpoint's size (no bucket-sized storages) that read back unchanged."""
     from gcbf_b200.synth import seeded_algo
-    ckpt = f'/root/reference/pretrained/{env_name}/models/step_500000'
+    ckpt = _checkpoint_like(env_name, str(tmp_path / 'ckpt'))
     env, algo = seeded_algo(env_name, 16, torch.device('cpu'))
     algo._ensure_bucket()                               # parameters become views into the flat bucket
     algo.load(ckpt)
@@ -125,11 +138,13 @@ def test_shipped_checkpoints_load_strictly(env_name, tmp_path):
         for k in want:
             assert torch.equal(sd[k], want[k]), k
     assert algo.cbf.feat_transformer.module_0.phi.net[2].weight_orig.data_ptr() >= algo._bucket.flat.data_ptr()   # still a bucket view
-    algo.save(str(tmp_path))
+    out = tmp_path / 'saved'
+    os.makedirs(out)
+    algo.save(str(out))
     for f, want in (('cbf.pkl', want_c), ('actor.pkl', want_a)):
-        size = os.path.getsize(tmp_path / f)
+        size = os.path.getsize(out / f)
         assert abs(size - os.path.getsize(os.path.join(ckpt, f))) < 65536, (f, size)      # not 2x: each file holds ONE net
-        back = torch.load(tmp_path / f, map_location='cpu')
+        back = torch.load(out / f, map_location='cpu')
         assert all(torch.equal(back[k], want[k]) for k in want)
 
 
@@ -196,7 +211,7 @@ def test_step_arena_views_are_disjoint_aligned_and_rewound():
 
 
 def test_tensor_core_dispatch_rule():
-    """Which layers of the reference's MLPs go to the tcgen05 kernel (host-side rule, no GPU needed)."""
+    """Which layers of the reference's MLPs go to the wgmma kernel (host-side rule, no GPU needed)."""
     from gcbf_b200 import ops
     assert ops.use_h(24196, 2048, 2048) and ops.use_h(8192, 1024, 2048) and ops.use_h(8192, 2048, 260)
     assert ops.use_h(24196, 128, 256)                       # gate 256 -> 128
@@ -404,7 +419,7 @@ def test_apply_entry_point_without_a_gpu():
 def test_abi_struct_mirrors_and_workspace_queries_without_a_gpu():
     """The ctypes mirrors of the chain-level ABI structures have the library's sizes, and the workspace queries (which replay a
     call's allocation sequence without launching) work on descriptors built from CPU tensors: sizes grow with the edge count and a
-    whole C3 step (~206 k edges, 65,536 agents) fits one B200 (180 GB) with room to spare."""
+    whole C3 step (~206 k edges, 65,536 agents) fits one H100 (80 GB) with room to spare."""
     from gcbf_b200 import synth
     from gcbf_b200.synth import seeded_algo
     mirrors = [_C.EnvCfg, native.LinearDesc, native.NetDesc, native.StepDesc, native.StepBatch, native.StepOut, native.NetCtx,

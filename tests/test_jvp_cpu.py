@@ -180,7 +180,7 @@ def jgrid():
     return ctypes.CDLL(so)
 
 
-GEOMETRIES = [(1, 1), (3, 7), (2, 256), (1184, 256)]       # one thread striding over everything ... more threads than work
+GEOMETRIES = [(1, 1), (3, 7), (2, 256), (1056, 256)]       # one thread striding over everything ... more threads than work
 
 
 @pytest.mark.parametrize('env_name,n,obs,B,area,seed,on_goal', CASES)

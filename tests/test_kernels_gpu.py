@@ -142,11 +142,11 @@ TC_SHAPES = [(256, 256, 96), (384, 128, 96), (1000, 2048, 2048), (2500, 256, 204
 
 @pytest.mark.parametrize('M,N,K', TC_SHAPES)
 def test_linear_tcgen05_3xfp16(M, N, K):
-    """tcgen05 path (forced) against fp64: forward with fused bias+ReLU, data grad with ReLU mask and accumulate, weight
+    """wgmma path (forced) against fp64: forward with fused bias+ReLU, data grad with ReLU mask and accumulate, weight
     grad + bias grad (fused into the split of dZ).  Tolerance 1e-5 of the output scale: the [hi|lo] fp16 companions carry
     22 significand bits and K is accumulated in 256-wide chunks promoted to fp32 registers (measured 1-2e-6)."""
-    if not _C.lib().gcbf_has_tcgen05():
-        pytest.skip('library built without the tcgen05 path')
+    if not _C.lib().gcbf_has_wgmma():
+        pytest.skip('library built without the wgmma path')
     g = _g(M + N + K)
     x, W, b = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g) / math.sqrt(K), torch.randn(N, generator=g)
     dz, rs = torch.randn(M, N, generator=g), torch.randn(M, K, generator=g)
@@ -550,7 +550,7 @@ def test_cbf_and_actor_forward_backward(env_name, n, obs, B, area):
 
 @pytest.mark.parametrize('impl,tol', [(1, 2e-5), (0, 3e-4)])
 def test_net_backward_exact_given_same_relu_masks(impl, tol):
-    """impl 1 = fp32 SIMT GEMMs (exact to fp32 round-off), impl 0 = tcgen05 3xFP16 where the shape qualifies (22-bit
+    """impl 1 = fp32 SIMT GEMMs (exact to fp32 round-off), impl 0 = wgmma 3xFP16 where the shape qualifies (22-bit
     operands; measured 1-2e-6 per GEMM, the tolerance below is the one the 3xTF32 predecessor needed).
     The whole fused backward (head -> gamma -> row scatter -> attention aggregation -> gate -> phi -> edge_attr,
     incl. the spectral-norm sigma term) against torch autograd in fp64 ON THE SAME ReLU MASKS (taken from the

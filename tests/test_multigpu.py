@@ -1,6 +1,6 @@
 """2-GPU data-parallel equality (SURVEY section 4 tier 6): two NCCL ranks, each owning half of the graphs, must produce
 the same losses and the same all-reduced gradient as one process on the concatenated batch.  Needs >= 2 visible GPUs
-(`gpurun --gpus 2 -- python -m pytest tests/test_multigpu.py -m gpu`)."""
+(`python -m pytest tests/test_multigpu.py -m gpu` on a machine with two GPUs)."""
 import os
 import socket
 

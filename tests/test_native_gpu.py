@@ -195,3 +195,26 @@ def test_apply_matches_python_sequencing(env_name, n, obs, area, rand, max_iter)
         assert na.abs().max().item() > 0                 # somebody violated: the refined action is not the nominal zero
     for x, y in zip(puv, nuv):                           # the same number of CBF passes -> the same number of power iterations
         assert torch.allclose(x, y, atol=1e-5)
+
+
+@pytest.mark.parametrize('env_name,n,obs,B,area,two_streams', [('DubinsCar', 64, 8, 4, 3.0, '0'), ('SimpleCar', 16, 0, 1, 4.0, '1'),
+                                                              ('SimpleDrone', 24, 24, 3, 1.0, '1')])
+def test_train_step_is_bit_reproducible(monkeypatch, env_name, n, obs, B, area, two_streams):
+    """Two runs of three train steps from the same seeded weights on the same batch give bit-identical results and weights:
+    reductions over blocks (split-K weight gradients, column sums, the edge-feature VJP) are summed in a fixed order, so the
+    result does not depend on block scheduling.  The cases cover the tensor-core layers (with emission), the few-rows kernels
+    of a single 16-agent graph, and the side stream."""
+    monkeypatch.setenv('GCBF_TWO_STREAMS', two_streams)
+    runs = []
+    for _ in range(2):
+        sb, env, algo, data = _setup(env_name, n, obs, B, area, 17)
+        for _ in range(3):
+            res = algo.train_step(data)
+        torch.cuda.synchronize()
+        out = {k: v.detach().clone() for k, v in res.items() if torch.is_tensor(v)}
+        out.update({'cbf.' + k: v.detach().clone() for k, v in algo.cbf.state_dict().items()})
+        out.update({'actor.' + k: v.detach().clone() for k, v in algo.actor.state_dict().items()})
+        runs.append(out)
+    assert runs[0].keys() == runs[1].keys()
+    for k in runs[0]:
+        assert torch.equal(runs[0][k], runs[1][k]), k

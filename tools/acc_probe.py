@@ -1,4 +1,4 @@
-"""Probe the tcgen05 fp32 accumulation: inputs on a binary grid (k/128, |k| <= 1023: 11-bit significands), i.e. exactly
+"""Probe the wgmma fp32 accumulation: inputs on a binary grid (k/128, |k| <= 1023: 11-bit significands), i.e. exactly
 representable by the fp16 hi plane under any power-of-two scale (lo = 0), while their products (22 bits) and sums are not
 representable in fp32, so every error of the tensor-core path is accumulation error.  With the
 256-wide chunk promotion the error must stay at the fp32 FFMA level for every K (without it: ~ -K/16 * 2^-24, truncation)."""

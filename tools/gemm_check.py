@@ -1,10 +1,10 @@
-"""GPU check of the tcgen05 3xFP16 GEMM against fp64 and against the fp32 SIMT kernel, plus timing of its pieces."""
+"""GPU check of the wgmma 3xFP16 GEMM against fp64 and against the fp32 SIMT kernel, plus timing of its pieces."""
 import sys, os, math, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [os.path.join(ROOT, 'gcbf-pytorch_b200')]
 from gcbf_b200 import ops, _C
 dev = torch.device('cuda:0')
-print('has tcgen05:', _C.lib().gcbf_has_tcgen05())
+print('has wgmma:', _C.lib().gcbf_has_wgmma())
 
 
 def run(M, N, K, impl, scale_x=1.0, scale_dz=1.0):
@@ -30,7 +30,7 @@ for shape in ACC_SHAPES:
         try:
             r2 = run(*shape, 2, sx, sdz)
             r1 = run(*shape, 1, sx, sdz)
-            print(shape, f'scales {sx:g}/{sdz:g}', 'tcgen05 err y/dx/dW/db: %.2e %.2e %.2e %.2e' % r2, '| simt: %.2e %.2e %.2e %.2e' % r1, flush=True)
+            print(shape, f'scales {sx:g}/{sdz:g}', 'wgmma err y/dx/dW/db: %.2e %.2e %.2e %.2e' % r2, '| simt: %.2e %.2e %.2e %.2e' % r1, flush=True)
         except Exception as ex:
             print(shape, 'FAILED', ex, flush=True)
 
@@ -48,7 +48,7 @@ def timeit(fn, n=5):
 
 print('GCBF_TC_KCH =', os.environ.get('GCBF_TC_KCH', 'default (4)'))
 for shape in [(1000, 2048, 2048), (70000, 128, 256)]:
-    print(shape, 'tcgen05 err y/dx/dW/db vs fp64: %.2e %.2e %.2e %.2e' % run(*shape, 2), flush=True)
+    print(shape, 'wgmma err y/dx/dW/db vs fp64: %.2e %.2e %.2e %.2e' % run(*shape, 2), flush=True)
 # timing at the real layer size (C2: E = 24,196 edges, 2048 x 2048 layer)
 ops.GEMM_IMPL = 0
 for (M, N, K) in [(24196, 2048, 2048), (8192, 2048, 2048), (24196, 256, 2048), (206139, 2048, 2048)]:

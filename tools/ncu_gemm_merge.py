@@ -1,6 +1,6 @@
 """Label an `ncu --set full -k regex:gemm_h_kernel` capture of tools/one_step.py with the (product, M, N, K) list the same command
-dumped -> profiles/r02_gemm_h_ncu_full.json (what bench.py's roofline.traffic looks up: DRAM bytes of exactly the dominant shape).
-    python tools/ncu_gemm_merge.py gpurun_out/gemm_C3.ncu-rep gpurun_out/shapes_C3.json profiles/r02_gemm_h_ncu_full.json"""
+dumped -> JSON with DRAM bytes and tensor-pipe use per labelled launch.
+    python tools/ncu_gemm_merge.py gemm_C3.ncu-rep shapes_C3.json gemm_C3.json"""
 import csv, json, subprocess, sys
 rep, shapes_path, out = sys.argv[1:4]
 raw = subprocess.run(['ncu', '-i', rep, '--page', 'raw', '--csv'], capture_output=True, text=True).stdout

@@ -3,8 +3,8 @@ aggregation, masks, losses, spectral norm, clip+Adam, fp16 split): achieved HBM 
 
     ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum,lts__t_bytes.sum --clock-control none \
         -k regex:'radius|edge_|attn_aggr|masks|loss|sn_|clip_adam|sumsq|split|amax|skinny|tiny|rows_|copy2d|step_|u_ref|pair_count|colsum' \
-        --csv --log-file gpurun_out/graphops_C3.csv python bench.py --steps 1 --warmup 1 --config C3 --also none --no-e2e --no-cpu-baseline
-    python tools/ncu_graphops.py gpurun_out/graphops_C3.csv profiles/r02_ncu_graphops_C3.json "C3: DubinsCar n=1024 obs=32 B=64"
+        --csv --log-file graphops_C3.csv python bench.py --steps 1 --warmup 1 --config C3 --also none --no-e2e --no-cpu-baseline
+    python tools/ncu_graphops.py graphops_C3.csv graphops_C3.json "C3: DubinsCar n=1024 obs=32 B=64"
 """
 import collections, csv, json, os, re, sys
 
@@ -14,7 +14,7 @@ try:
     peak = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs']
     peak_src = 'MEASURED_PEAKS.json hbm_gbs'
 except Exception:
-    peak, peak_src = 6650.0, 'fallback (B200_PROFILING.md)'
+    peak, peak_src = 3350.0, 'H100 SXM data sheet (not measured)'
 with open(src) as f:
     lines = [l for l in f if not l.startswith('==')]
 per = collections.defaultdict(dict)            # launch id -> metric -> value
@@ -51,7 +51,7 @@ for k, a in sorted(agg.items(), key=lambda kv: -kv[1]['seconds']):
                      best_launch_hbm_GBs=round(a['best_gbs'], 1), best_launch=a['best_launch']))
 json.dump(dict(workload=label, hbm_peak_GBs=peak, peak_source=peak_src,
                note='ncu per-launch values are cold-cache and serialised (--clock-control none); DRAM bytes = dram__bytes_read.sum + dram__bytes_write.sum; '
-                    'kernels whose working set fits the 126 MB L2 (a graph\'s positions are <= 68 KB) show little DRAM traffic by design: their l2_GBs is the relevant rate',
+                    'kernels whose working set fits the 50 MB L2 (a graph\'s positions are <= 68 KB) show little DRAM traffic by design: their l2_GBs is the relevant rate',
                kernels=rows), open(out, 'w'), indent=1)
 print(f'{len(rows)} kernels -> {out}')
 for r in rows[:14]:
