@@ -1,16 +1,19 @@
-// GCBF.apply, the test-time controller (reference gcbf/algo/gcbf.py:260-309), as ONE C-ABI call for one graph:
+// GCBF.apply, the test-time controller (reference gcbf/algo/gcbf.py:260-309), as ONE C-ABI call for B graphs at once:
 //
 //   h = cbf(graph) [:262], action = actor(graph) [:263], h_next = cbf(forward_graph(graph, 0)) [:264-267]; agents whose nominal (zero)
 //   action satisfies the h_dot condition keep it [:271-273]; then up to max_iter + 1 rounds of
 //       h_next = cbf(forward_graph(graph, action)) [:288-290], max_val = relu(-h_dot - alpha h) [:291-292],
-//       stop when nobody violates or the round counter passed max_iter [:294],
-//       d mean(max_val) / d action through the CBF net's input-gradient path (no weight gradient) [:300],
+//       a graph is done when none of its agents violates or the round counter passed max_iter [:294],
+//       d mean_g(max_val) / d action through the CBF net's input-gradient path (no weight gradient) [:300],
 //       one Adam(lr) step per VIOLATING agent (its own step count) [:298-302] + the gradient-proportional noise [:305].
 //
-// The reference keeps one torch.optim.Adam per agent; here the per-agent optimiser state is three small arrays (m, v, step count) and
-// one kernel updates every violating agent.  Each round costs one host sync (the violating-agent count decides whether the backward is
-// launched at all), like the reference's `if loss_h_dot <= 0` [:294].  Every CBF pass advances the spectral-norm vectors (the reference
-// never calls .eval(), SURVEY 3.5).
+// Every piece of the loop's state is per agent (action, Adam moments, step count) or per graph (done flag, round count), and the GNN
+// passes are block-diagonal, so graph g of a batch computes exactly what a call on graph g alone computes: a done graph keeps its
+// action, gets no Adam step and is not re-evaluated, while the other graphs go on.  The reference keeps one torch.optim.Adam per
+// agent; here the per-agent optimiser state is three small arrays (m, v, step count) and one kernel updates every violating agent.
+// Each round costs one host sync (the number of graphs still refining decides whether the backward is launched at all), like the
+// reference's `if loss_h_dot <= 0` [:294].  Every CBF pass advances the spectral-norm vectors (the reference never calls .eval(),
+// SURVEY 3.5); a batch makes the passes of its slowest graph, in the same order.  gcbf_apply is the one-graph case.
 #include <cstdlib>
 
 #include "chain.h"
@@ -33,21 +36,52 @@ __global__ void apply_init_kernel(const float* __restrict__ h, const float* __re
   if (i % a == 0) t[r] = 0.f;
 }
 
-// max_val = relu(-h_dot - alpha h), d mean(max_val) / d h_next, number of violating agents
-__global__ void apply_viol_kernel(const float* __restrict__ h, const float* __restrict__ hn, float* __restrict__ max_val,
-                                  float* __restrict__ d_hn, int* __restrict__ count, int M, float dt, float alpha) {
+// max_val = relu(-h_dot - alpha h) of the graphs still refining (0 for done graphs), d mean_g(max_val) / d h_next (n = agents per graph),
+// violating agents per graph.  Integer atomics: the counts do not depend on the order (warps straddle graphs when n < 32)
+__global__ void apply_viol_kernel(const float* __restrict__ h, const float* __restrict__ hn, const int* __restrict__ done,
+                                  float* __restrict__ max_val, float* __restrict__ d_hn, int* __restrict__ graph_count, int M, int n,
+                                  float dt, float alpha) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  bool on = false;
-  if (i < M) {
+  if (i >= M) return;
+  const int g = i / n;
+  float mv = 0.f;
+  if (!done[g]) {
     const float hd = __fdiv_rn(__fsub_rn(hn[i], h[i]), dt);
-    const float mv = fmaxf(__fsub_rn(-hd, __fmul_rn(alpha, h[i])), 0.f);
-    max_val[i] = mv;
-    on = mv > 0.f;
-    d_hn[i] = on ? -1.f / (dt * (float)M) : 0.f;
+    mv = fmaxf(__fsub_rn(-hd, __fmul_rn(alpha, h[i])), 0.f);
   }
-  const unsigned b = __ballot_sync(0xffffffffu, on);
-  if ((threadIdx.x & 31) == 0 && b) atomicAdd(count, __popc(b));
-  if (i == 0) count[1] += 1;      // rounds evaluated so far: the Adam kernel of this round reads noise slice count[1] - 1
+  max_val[i] = mv;
+  const bool on = mv > 0.f;
+  d_hn[i] = on ? -1.f / (dt * (float)n) : 0.f;
+  if (on) atomicAdd(graph_count + g, 1);
+}
+
+// after round `count[1]` was evaluated: a graph with no violating agent, or any graph once the round counter passed max_iter, is done
+// (rounds[g] = the Adam rounds it did); count[0] = graphs still refining (what the host reads), count[1] += 1 (the Adam kernel of this
+// round reads noise slice count[1] - 1).  One block; the per-graph counts are cleared for the next round.
+__global__ void apply_done_kernel(int* __restrict__ done, int* __restrict__ graph_count, int32_t* __restrict__ rounds,
+                                  int* __restrict__ count, int G, int max_iter) {
+  __shared__ int active;
+  if (threadIdx.x == 0) active = 0;
+  __syncthreads();
+  const int it = count[1];
+  int mine = 0;
+  for (int g = threadIdx.x; g < G; g += blockDim.x) {
+    if (!done[g]) {
+      if (graph_count[g] == 0 || it > max_iter) {
+        done[g] = 1;
+        rounds[g] = it;
+      } else {
+        ++mine;
+      }
+    }
+    graph_count[g] = 0;
+  }
+  if (mine) atomicAdd(&active, mine);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    count[0] = active;
+    count[1] = it + 1;
+  }
 }
 
 // torch.optim.Adam(lr, betas (0.9, 0.999), eps 1e-8) on the rows with max_val != 0, each with its own step count, then
@@ -79,7 +113,9 @@ __global__ void agent_adam_kernel(float* __restrict__ act, float* __restrict__ m
 struct ApplyBufs {
   float *h, *actor_action, *hn, *act, *m, *v, *t, *max_val, *d_hn, *zero_action, *states_next, *ea_next, *g, *d_ea, *d_states;
   uint8_t* pass_mask;
-  int* count;
+  int* count;                     // [0] graphs still refining after the round, [1] rounds evaluated
+  int *done, *graph_count;        // per graph
+  int32_t* rounds;                // per graph: the caller's array, or workspace for gcbf_apply
 };
 
 static int* g_pinned_count = nullptr;
@@ -90,17 +126,20 @@ static int apply_forward(Run& R, const gcbf_step_desc& d, const gcbf_step_batch&
   const int M = b.num_agents_total, Nn = b.num_nodes, E = (int)b.num_edges, s = d.state_dim;
   gcbf_env_cfg cfg = d.env;
   if (!R.dry) {
-    // a single graph: the reach-freeze branch of forward_graph (dubins_car.py:126)
-    CHAIN_CALL(gcbf_step_fwd(&cfg, b.states, b.ld_state, action, d.goal, d.ld_goal, d.lqr_gain, 1, B.states_next, B.pass_mask, R.st));
+    // every graph is a single graph of the reference: the reach-freeze branch of forward_graph (dubins_car.py:126), per graph
+    CHAIN_CALL((d.goal_per_graph ? gcbf_step_fwd_multi : gcbf_step_fwd)(&cfg, b.states, b.ld_state, action, d.goal, d.ld_goal, d.lqr_gain, 1,
+                                                                        B.states_next, B.pass_mask, R.st));
     CHAIN_CALL(gcbf_edge_attr_fwd(d.env.env, B.states_next, s, b.edge_index, E, B.ea_next, R.st));
     R.launched(E ? 2 : 1);
   }
   return net_forward(R, cbf, b.x, B.ea_next, b.edge_index, b.rowptr, E, Nn, b.row_index, M, nullptr, B.hn, 1, ctx);
 }
 
+// rounds: device int32[num_graphs] or NULL (workspace); *iterations (optional): rounds of the slowest graph
 static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, float lr, float rand, const float* noise, int max_iter,
-                     float* action_out, int ld_action, int* iterations) {
+                     float* action_out, int ld_action, int32_t* rounds, int* iterations, const char* what) {
   const int M = b.num_agents_total, Nn = b.num_nodes, E = (int)b.num_edges, a = d.action_dim, s = d.state_dim, ed = d.cbf.edge_dim;
+  const int G = d.env.num_graphs, n = d.env.num_agents;
   const float dt = (float)d.env.dt;
   ApplyBufs B;
   B.h = (float*)R.ws.alloc((size_t)M * 4);
@@ -116,6 +155,10 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
   B.zero_action = (float*)R.ws.alloc((size_t)M * a * 4);
   B.pass_mask = (uint8_t*)R.ws.alloc((size_t)M * a);
   B.count = (int*)R.ws.alloc(256);
+  B.done = (int*)R.ws.alloc((size_t)G * 4 * 2);
+  B.graph_count = B.done + G;
+  B.rounds = (int32_t*)R.ws.alloc((size_t)G * 4);
+  if (rounds) B.rounds = rounds;
   B.states_next = (float*)R.ws.alloc((size_t)Nn * s * 4);
   B.d_states = (float*)R.ws.alloc((size_t)Nn * s * 4);
   B.ea_next = (float*)R.ws.alloc((size_t)E * ed * 4);
@@ -123,7 +166,7 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
   gcbf_net_desc cbf_again = d.cbf;
   cbf_again.refresh_weights = 0;
   gcbf_env_cfg cfg = d.env;
-  const int grid_ma = ceil_div(M * a, 256), grid_m = ceil_div(M, 256);
+  const int grid_ma = ceil_div(M * a, 256), grid_m = ceil_div(M, 256), block_g = G < 256 ? 32 * ceil_div(G, 32) : 256;
   const size_t mark0 = R.ws.off;
   if (int rc = net_forward(R, d.cbf, b.x, b.edge_attr, b.edge_index, b.rowptr, E, Nn, b.row_index, M, nullptr, B.h, 1, nullptr)) return rc;            // :262
   size_t peak = R.ws.off;
@@ -140,7 +183,7 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
     GCBF_LAUNCH_OK();
     R.launched(2);
   }
-  // One round = two launch sequences around the host's look at the violating-agent count.  Every round of a call launches exactly the
+  // One round = two launch sequences around the host's look at the number of graphs still refining.  Every round of a call launches exactly the
   // same kernels on the same pointers (the workspace is rewound, the noise slice is picked on the device), so round 1 is captured into
   // two CUDA graphs that rounds 2.. replay: ~75 dependent launches of a few microseconds each become two graph launches.  Round 0 runs
   // eagerly (one-time attribute / descriptor set-up happens there); GCBF_APPLY_GRAPH=0, per-launch timing or a failed capture keep the
@@ -149,11 +192,12 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
   auto round_fwd = [&]() -> int {
     if (int rc = apply_forward(R, d, b, cbf_again, B, B.act, &ctx)) return rc;                                                                          // :288-290
     if (!R.dry) {
-      CHAIN_CUDA(cudaMemsetAsync(B.count, 0, 4, R.st));
-      apply_viol_kernel<<<grid_m, 256, 0, R.st>>>(B.h, B.hn, B.max_val, B.d_hn, B.count, M, dt, d.alpha);                                               // :291-293
+      apply_viol_kernel<<<grid_m, 256, 0, R.st>>>(B.h, B.hn, B.done, B.max_val, B.d_hn, B.graph_count, M, n, dt, d.alpha);                              // :291-293
+      GCBF_LAUNCH_OK();
+      apply_done_kernel<<<1, block_g, 0, R.st>>>(B.done, B.graph_count, B.rounds, B.count, G, max_iter);                                                // :294
       GCBF_LAUNCH_OK();
       CHAIN_CUDA(cudaMemcpyAsync(g_pinned_count, B.count, 4, cudaMemcpyDeviceToHost, R.st));
-      R.launched(2);
+      R.launched(3);
     }
     return 0;
   };
@@ -202,7 +246,10 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
     if (gf.exec) cudaGraphExecDestroy(gf.exec);
     if (gb.exec) cudaGraphExecDestroy(gb.exec);
   };
-  if (!R.dry) CHAIN_CUDA(cudaMemsetAsync(B.count, 0, 8, R.st));      // [0] violating agents of the round, [1] rounds evaluated
+  if (!R.dry) {
+    CHAIN_CUDA(cudaMemsetAsync(B.count, 0, 8, R.st));                  // [0] graphs still refining, [1] rounds evaluated
+    CHAIN_CUDA(cudaMemsetAsync(B.done, 0, (size_t)G * 4 * 2, R.st));   // done flags, per-graph violating counts
+  }
   int it = 0;
   for (;; ++it) {
     int rc = 0;
@@ -211,8 +258,8 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
     else rc = round_fwd();
     if (rc) { cleanup(); return rc; }
     if (!R.dry) {
-      if (cudaStreamSynchronize(R.st) != cudaSuccess) { cleanup(); set_error("gcbf_apply: %s", cudaGetErrorString(cudaGetLastError())); return GCBF_E_CUDA; }
-      if (*g_pinned_count == 0 || it > max_iter) break;                                                                                                 // :294
+      if (cudaStreamSynchronize(R.st) != cudaSuccess) { cleanup(); set_error("%s: %s", what, cudaGetErrorString(cudaGetLastError())); return GCBF_E_CUDA; }
+      if (*g_pinned_count == 0 || it > max_iter) break;                // every graph done (past max_iter all of them are)    :294
     }
     if (graphs && gb.exec) { rc = cudaGraphLaunch(gb.exec, R.st) == cudaSuccess ? 0 : GCBF_E_CUDA; R.launched((int)gb.launches); }
     else if (graphs && it == 1) rc = capture_and_launch(gb, round_bwd);
@@ -235,25 +282,52 @@ static int apply_run(Run& R, const gcbf_step_desc& d, const gcbf_step_batch& b, 
 using namespace gcbf;
 using namespace gcbf::chain;
 
-extern "C" size_t gcbf_apply_workspace_bytes(const gcbf_step_desc* d, const gcbf_step_batch* g) {
-  if (check_step(d, g, "gcbf_apply_workspace_bytes")) return 0;
+static size_t apply_workspace(const gcbf_step_desc* d, const gcbf_step_batch* g, const char* what) {
+  if (check_step(d, g, what)) return 0;
   Run R(nullptr, 0, nullptr, true);
-  if (apply_run(R, *d, *g, 0.f, 0.f, nullptr, 0, nullptr, 0, nullptr)) return 0;
+  if (apply_run(R, *d, *g, 0.f, 0.f, nullptr, 0, nullptr, 0, nullptr, nullptr, what)) return 0;
   return R.ws.off + 4096;
+}
+
+// the checks both entry points make before any CUDA call
+static int apply_check(const gcbf_step_desc* d, const gcbf_step_batch* g, float lr, float rand, const float* noise, int max_iter,
+                       const float* action, int ld_action, void* workspace, size_t workspace_bytes, const char* what) {
+  GCBF_REQUIRE(action && ld_action >= d->action_dim && max_iter >= 0 && lr > 0.f && workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
+               "%s: bad arguments", what);
+  GCBF_REQUIRE(rand == 0.f || noise, "%s: rand != 0 needs the noise array [(max_iter + 1), num_agents, action_dim]", what);
+  GCBF_REQUIRE(g->states && g->x && g->rowptr && g->u_ref && d->goal && (g->num_edges == 0 || (g->edge_attr && g->edge_index)), "%s: null pointer", what);
+  const size_t need = apply_workspace(d, g, what);
+  if (need == 0) return GCBF_E_INVALID;
+  if (need > workspace_bytes) { set_error("%s: workspace too small (%zu needed, %zu given)", what, need, workspace_bytes); return GCBF_E_WORKSPACE; }
+  if (!g_pinned_count) GCBF_CUDA_OK(cudaHostAlloc(&g_pinned_count, 64, cudaHostAllocDefault));
+  return 0;
+}
+
+extern "C" size_t gcbf_apply_workspace_bytes(const gcbf_step_desc* d, const gcbf_step_batch* g) {
+  return apply_workspace(d, g, "gcbf_apply_workspace_bytes");
 }
 
 extern "C" int gcbf_apply(const gcbf_step_desc* d, const gcbf_step_batch* g, float lr, float rand, const float* noise, int max_iter,
                           float* action, int ld_action, int* iterations, void* workspace, size_t workspace_bytes, void* stream) {
   if (int rc = check_step(d, g, "gcbf_apply")) return rc;
   GCBF_REQUIRE(d->env.num_graphs == 1 && !d->goal_per_graph, "gcbf_apply: one graph per call (gcbf.py:260 takes a single Data)");
-  GCBF_REQUIRE(action && ld_action >= d->action_dim && max_iter >= 0 && lr > 0.f && workspace && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0,
-               "gcbf_apply: bad arguments");
-  GCBF_REQUIRE(rand == 0.f || noise, "gcbf_apply: rand != 0 needs the noise array [(max_iter + 1), num_agents, action_dim]");
-  GCBF_REQUIRE(g->states && g->x && g->rowptr && g->u_ref && d->goal && (g->num_edges == 0 || (g->edge_attr && g->edge_index)), "gcbf_apply: null pointer");
-  const size_t need = gcbf_apply_workspace_bytes(d, g);
-  if (need > workspace_bytes) { set_error("gcbf_apply: workspace too small (%zu needed, %zu given)", need, workspace_bytes); return GCBF_E_WORKSPACE; }
-  if (!g_pinned_count) GCBF_CUDA_OK(cudaHostAlloc(&g_pinned_count, 64, cudaHostAllocDefault));
+  if (int rc = apply_check(d, g, lr, rand, noise, max_iter, action, ld_action, workspace, workspace_bytes, "gcbf_apply")) return rc;
   Run R(workspace, workspace_bytes, as_stream(stream), false);
-  int rc = apply_run(R, *d, *g, lr, rand, rand != 0.f ? noise : nullptr, max_iter, action, ld_action, iterations);
+  int rc = apply_run(R, *d, *g, lr, rand, rand != 0.f ? noise : nullptr, max_iter, action, ld_action, nullptr, iterations, "gcbf_apply");
   return R.finish(rc, "gcbf_apply");
+}
+
+extern "C" size_t gcbf_apply_batch_workspace_bytes(const gcbf_step_desc* d, const gcbf_step_batch* batch) {
+  return apply_workspace(d, batch, "gcbf_apply_batch_workspace_bytes");
+}
+
+extern "C" int gcbf_apply_batch(const gcbf_step_desc* d, const gcbf_step_batch* batch, float lr, float rand, const float* noise, int max_iter,
+                                float* action, int ld_action, int32_t* rounds, int* iterations, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+  if (int rc = check_step(d, batch, "gcbf_apply_batch")) return rc;      // num_agents_total / num_nodes against num_graphs x the per-graph sizes
+  GCBF_REQUIRE(rounds, "gcbf_apply_batch: rounds (device int32[num_graphs]) is required");
+  if (int rc = apply_check(d, batch, lr, rand, noise, max_iter, action, ld_action, workspace, workspace_bytes, "gcbf_apply_batch")) return rc;
+  Run R(workspace, workspace_bytes, as_stream(stream), false);
+  int rc = apply_run(R, *d, *batch, lr, rand, rand != 0.f ? noise : nullptr, max_iter, action, ld_action, rounds, iterations, "gcbf_apply_batch");
+  return R.finish(rc, "gcbf_apply_batch");
 }

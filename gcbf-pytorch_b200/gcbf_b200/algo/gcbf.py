@@ -480,31 +480,58 @@ class GCBF(Algorithm):
         plus the reference's gradient noise `rand * lr * randn * grad`.  The per-agent optimisers are kept as one
         vectorised state (m, v, step count per agent); the O(num_agents) arithmetic around the kernels is host glue."""
         if ops.NATIVE and data.states.is_cuda:
-            return self._apply_native(data, rand, max_iter)
+            return self._apply_native(data, rand, max_iter, None, batched=False)
+        return self._apply_python(data, rand, max_iter, None)
+
+    def apply_batch(self, batch, rand: Optional[float] = 30, max_iter: int = 30, noise: Optional[Tensor] = None) -> Tensor:
+        """`apply` for every graph of a collated batch of B graphs (with `u_ref`; optional per-graph goal sets in `batch.goal`
+        [B * n, goal_dim]) in one call: graph g gets exactly what `apply` on graph g alone gives -- its own termination, its own
+        per-agent Adam state, the mean of its loss over its own agents.  Returns the actions [B * n, action_dim]; the Adam rounds each
+        graph did go to `self.last_apply_batch_rounds` (host int tensor [B]).  noise: the standard normals of the gradient noise
+        [(max_iter + 1), B * n, action_dim] (default: drawn here); round k of graph g reads its rows of slice k, so concatenated
+        per-graph draws reproduce per-graph calls."""
+        if ops.NATIVE and batch.states.is_cuda:
+            return self._apply_native(batch, rand, max_iter, noise, batched=True)
+        return self._apply_python(batch, rand, max_iter, noise)
+
+    def _apply_python(self, data, rand: Optional[float], max_iter: int, noise: Optional[Tensor]) -> Tensor:
+        """The Python-sequenced controller (autograd over the per-kernel ops) for B >= 1 graphs: per-graph done flags and loss means,
+        per-agent Adam state."""
         env, alpha, lr = self._env, float(self.params['alpha']), 0.1
         dt = float(env.dt)
+        B, n = env._num_graphs_of(data), env.num_agents
+        goal = getattr(data, 'goal', None) if hasattr(data, 'goal') else None
         with torch.no_grad():
             h = self.cbf(data)
             action = self.actor(data)
             nominal = torch.zeros_like(action)
-            h_next = self.cbf(env.forward_graph(data, nominal))
+            h_next = self.cbf(env.forward_graph(data, nominal, single=True, goal=goal))
             viol = torch.relu(-(h_next - h) / dt - alpha * h).reshape(-1)
             act = torch.where((viol <= 0).unsqueeze(1), nominal, action).clone()
         m, v = torch.zeros_like(act), torch.zeros_like(act)
         t = torch.zeros(act.shape[0], device=act.device)
-        noise = torch.randn(max_iter + 1, *act.shape, device=act.device) if rand else None     # one draw, like the library path
+        if rand and noise is None:
+            noise = torch.randn(max_iter + 1, *act.shape, device=act.device)     # one draw, like the library path
+        done = torch.zeros(B, dtype=torch.bool, device=act.device)
+        rounds = torch.zeros(B, dtype=torch.int64)
         it = 0
         while True:
             a = act.clone().requires_grad_(True)
-            h_next = self.cbf(env.forward_graph(data, a))
-            max_val = torch.relu(-(h_next - h) / dt - alpha * h)
-            loss = torch.mean(max_val)
-            if float(loss.detach()) <= 0 or it > max_iter:
+            h_next = self.cbf(env.forward_graph(data, a, single=True, goal=goal))
+            max_val = torch.relu(-(h_next - h) / dt - alpha * h).reshape(B, n)
+            max_val = torch.where(done.unsqueeze(1), torch.zeros_like(max_val), max_val)   # a done graph is not re-evaluated
+            loss = max_val.mean(dim=1)                                                       # per graph: mean over its agents
+            finished = ~done & ((loss.detach() <= 0) | (it > max_iter))
+            rounds[finished.cpu()] = it
+            done = done | finished
+            if bool(done.all()):
+                self.last_apply_batch_rounds = rounds
+                self.last_apply_rounds = int(rounds.max())
                 return a.detach()
             sel = (max_val.detach().reshape(-1) != 0)
             ops.SKIP_WGRAD = True           # only d loss / d action is needed: skip every weight-gradient GEMM
             try:
-                (g,) = torch.autograd.grad(loss, a)
+                (g,) = torch.autograd.grad(loss.sum(), a)                    # graphs are independent: d sum_g loss_g / d a_g = d loss_g / d a_g
             finally:
                 ops.SKIP_WGRAD = False
             with torch.no_grad():
@@ -519,25 +546,33 @@ class GCBF(Algorithm):
                     act = torch.where(s2, act - rand * lr * noise[it] * g, act)
             it += 1
 
-    def _apply_native(self, data, rand: Optional[float], max_iter: int) -> Tensor:
-        """The same controller as ONE library call (gcbf_apply, csrc/apply.cu): the whole refinement loop, the per-agent Adam
-        kernel and the termination test run inside the library; this method only draws the noise and hands over pointers."""
+    def _apply_native(self, data, rand: Optional[float], max_iter: int, noise: Optional[Tensor], batched: bool) -> Tensor:
+        """The same controller as ONE library call (gcbf_apply / gcbf_apply_batch, csrc/apply.cu): the whole refinement loop, the
+        per-agent Adam kernel and the termination test run inside the library; this method only draws the noise and hands over
+        pointers."""
         import ctypes
         from .. import native
         dev = data.states.device
         d, b, _alive, cbf_layers, act_layers, M, E = self._native_inputs(data)
         a = self.action_dim
-        need = native.fn('gcbf_apply_workspace_bytes')(ctypes.byref(d), ctypes.byref(b))
+        name = 'gcbf_apply_batch' if batched else 'gcbf_apply'
+        need = native.fn(name + '_workspace_bytes')(ctypes.byref(d), ctypes.byref(b))
         if need == 0:
-            native.check(-1, 'gcbf_apply_workspace_bytes')
+            native.check(-1, name + '_workspace_bytes')
         buf = getattr(self, '_apply_ws', None)
         if buf is None:
             buf = self._apply_ws = native.GrowBuffer()
         ws = buf.get(need, dev)
         rand = float(rand) if rand else 0.0
-        noise = torch.randn(max_iter + 1, M, a, device=dev) if rand else None      # gcbf.py:305 draws randn_like per agent and round
+        if rand and noise is None:
+            noise = torch.randn(max_iter + 1, M, a, device=dev)      # gcbf.py:305 draws randn_like per agent and round
+        if noise is not None:
+            if tuple(noise.shape) != (max_iter + 1, M, a):
+                raise ValueError(f'noise must be [{max_iter + 1}, {M}, {a}], got {tuple(noise.shape)}')
+            noise = noise.to(dev, torch.float32).contiguous()
         action = torch.empty(M, a, device=dev)
         rounds = ctypes.c_int(0)
+        graph_rounds = torch.empty(d.env.num_graphs, device=dev, dtype=torch.int32) if batched else None
         # the library captures a round into CUDA graphs and replays it; capture is impossible on the legacy default stream, so the call
         # runs on a stream of its own, ordered after and before the caller's stream
         cur = torch.cuda.current_stream(dev)
@@ -545,14 +580,21 @@ class GCBF(Algorithm):
         if st is None or st.device != dev:
             st = self._apply_stream = torch.cuda.Stream(dev)
         st.wait_stream(cur)
+        noise_ptr = noise.data_ptr() if (rand and noise is not None) else None
         with torch.cuda.stream(st):
-            rc = native.fn('gcbf_apply')(ctypes.byref(d), ctypes.byref(b), 0.1, rand, noise.data_ptr() if noise is not None else None,
-                                         int(max_iter), action.data_ptr(), a, ctypes.byref(rounds), ws.data_ptr(), ws.numel(), st.cuda_stream)
+            if batched:
+                rc = native.fn(name)(ctypes.byref(d), ctypes.byref(b), 0.1, rand, noise_ptr, int(max_iter), action.data_ptr(), a,
+                                     graph_rounds.data_ptr(), ctypes.byref(rounds), ws.data_ptr(), ws.numel(), st.cuda_stream)
+            else:
+                rc = native.fn(name)(ctypes.byref(d), ctypes.byref(b), 0.1, rand, noise_ptr, int(max_iter), action.data_ptr(), a,
+                                     ctypes.byref(rounds), ws.data_ptr(), ws.numel(), st.cuda_stream)
         cur.wait_stream(st)
-        native.check(rc, 'gcbf_apply')
+        native.check(rc, name)
         native._mark_fresh(cbf_layers)
         native._mark_fresh(act_layers)
         self.last_apply_rounds = rounds.value
+        if batched:
+            self.last_apply_batch_rounds = graph_rounds.cpu().to(torch.int64)
         return action
 
     # ---- analytic h_dot (SURVEY section 8f-3; additive: the training loss keeps the reference's finite difference) ------------------

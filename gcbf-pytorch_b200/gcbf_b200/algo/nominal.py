@@ -29,3 +29,8 @@ class Nominal(Algorithm):
 
     def apply(self, data, rand: Optional[float] = 30) -> Tensor:
         return self.act(data)
+
+    def apply_batch(self, batch, rand: Optional[float] = 30, max_iter: int = 30, noise: Optional[Tensor] = None) -> Tensor:
+        """The nominal action for every graph of a collated batch (nothing to refine: zero rounds per graph)."""
+        self.last_apply_batch_rounds = torch.zeros(self._env._num_graphs_of(batch), dtype=torch.int64)
+        return self.act(batch)

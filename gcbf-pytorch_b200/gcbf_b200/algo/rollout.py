@@ -14,7 +14,7 @@ within dist2goal of their goals (checked on the device; the flags are read back 
 env may run a few extra steps before it is re-sampled -- its agents are frozen at their goals by then).
 """
 import ctypes
-from typing import Dict, Optional
+from typing import Callable, Dict, Optional, Sequence
 
 import numpy as np
 import torch
@@ -62,11 +62,29 @@ class VectorRollout:
             self.t[i] = 0
 
     # ---- one vectorised step ------------------------------------------------------------------------------------------------
-    @torch.no_grad()
-    def step(self, prob: float = 0.0, store: bool = True) -> Dict[str, torch.Tensor]:
+    def keep(self, which):
+        """Keep only the environments `which` (ascending indices into the current batch), in that order: the others drop out of the
+        batch and cost nothing from the next step on."""
+        idx = torch.as_tensor(np.asarray(which, dtype=np.int64))
+        nodes = (idx.unsqueeze(1) * self.N + torch.arange(self.N)).reshape(-1).to(self.dev)
+        agents = (idx.unsqueeze(1) * self.n + torch.arange(self.n)).reshape(-1).to(self.dev)
+        self.states = self.states[nodes].contiguous()
+        self.goals = self.goals[agents].contiguous()
+        self.t = self.t[idx.numpy()]
+        self.B = int(idx.numel())
+        self._done_host = None
+
+    def step(self, prob: float = 0.0, store: bool = True, policy: Optional[Callable] = None) -> Dict[str, torch.Tensor]:
         """All envs advance one step under the actor (each env's action zeroed with probability `prob`, the reference's
-        exploration schedule gcbf.py:131-132).  Returns device tensors: reach [B, n], collision [B, n] (after the step),
-        is_safe [B] (before the step: what the stored graph is labelled with, gcbf.py:133-137)."""
+        exploration schedule gcbf.py:131-132), or under `policy(batch)` -- e.g. `algo.apply_batch`, the test-time controller --
+        which gets the collated batch with u_ref and the per-env goal sets (`batch.goal`).  Returns device tensors: reach [B, n],
+        collision [B, n] (after the step), is_safe [B] (before the step: what the stored graph is labelled with, gcbf.py:133-137)."""
+        if policy is None:
+            with torch.no_grad():
+                return self._step(prob, store, None)
+        return self._step(prob, store, policy)
+
+    def _step(self, prob: float, store: bool, policy: Optional[Callable]) -> Dict[str, torch.Tensor]:
         env, B, n, N = self.env, self.B, self.n, self.N
         cfg = env._cfg(B)
         st, ld = ops._mat(self.states)
@@ -76,7 +94,11 @@ class VectorRollout:
         _C.call('gcbf_u_ref_multi', ctypes.byref(cfg), _C.ptr(st), ld, _C.ptr(goal), ldg, _C.ptr(env._gain()), _C.ptr(u_ref))
         data = env.add_communication_links(env.make_graph(self.states))          # ONE radius graph + edge features for all envs
         data.update(Data(u_ref=u_ref))
-        action = self.algo.actor(data)                                           # ONE actor forward (block-diagonal batch)
+        if policy is None:
+            action = self.algo.actor(data)                                       # ONE actor forward (block-diagonal batch)
+        else:
+            data.update(Data(goal=self.goals))
+            action = policy(data).detach()
         if prob > 0:
             keep = torch.from_numpy((np.random.rand(B) >= prob).astype(np.float32)).to(self.dev, non_blocking=True)
             action = action * keep.repeat_interleave(n).unsqueeze(1)
@@ -120,3 +142,74 @@ class VectorRollout:
         if timeout:
             self.reset(timeout)
         return dict(reach=reach, collision=collision, is_safe=is_safe, action=action, edge_count=int(data.edge_index.shape[1]))
+
+
+def evaluate_episodes(env, algo, seeds: Sequence[int], rand: Optional[float] = 30, max_iter: int = 30,
+                      max_steps: Optional[int] = None) -> Dict[str, object]:
+    """Test-time evaluation episodes (reference gcbf/trainer/utils.py:127-223 `eval_ctrl_epi`, one episode per seed) stepped as ONE
+    batch: per step, u_ref for every live episode, `algo.apply_batch` (the test-time controller over all of them at once), the dynamics
+    with the single-graph reach-freeze branch, the radius graph, reach / collision and the env's per-agent reward.
+
+    Initial states and goals come from `set_seed(seed); env.reset()`, one seed after another, so they are those of a sequential
+    evaluation with the same seeds.  An episode ends when its step count reaches `max_steps` (default env.max_episode_steps) or all its
+    agents are at their goals; it then drops out of the batch and its statistics stay as they were at its last step.
+
+    Returns per-episode numpy arrays `reward` (sum over steps of the mean agent reward), `length`, `safe` (fraction of agents that never
+    collided), `reach` (fraction at their goals at the end) and `success` (both), and `mean` / `std` of each over the episodes (what
+    the reference's test.py prints), and every episode's last states `final_states` [S, nodes_per_graph, state_dim]."""
+    from ..trainer.utils import set_seed
+    from .macbf import MACBF
+    if isinstance(algo, MACBF):
+        raise NotImplementedError('evaluate_episodes: MACBF has no batched test-time controller; evaluate it one episode at a time')
+    if not hasattr(algo, 'apply_batch'):
+        raise NotImplementedError(f'evaluate_episodes: {type(algo).__name__} has no apply_batch')
+    seeds = [int(s) for s in seeds]
+    S, n, N, pd = len(seeds), env.num_agents, env.nodes_per_graph, env.POS_DIM
+    max_steps = int(env.max_episode_steps if max_steps is None else max_steps)
+    states, goals = [], []
+    for s in seeds:
+        set_seed(s)
+        data = env.reset()
+        states.append(data.states.detach().clone())
+        goals.append(env._goal.detach().clone())
+    vr = VectorRollout(env, algo, S, states=torch.cat(states), goals=torch.cat(goals))
+    dev, d2g = vr.dev, env._params['dist2goal']
+    reward = torch.zeros(S, device=dev, dtype=torch.float64)
+    length = np.zeros(S, dtype=np.int64)
+    safe = torch.ones(S, n, device=dev, dtype=torch.bool)
+    reach = torch.zeros(S, n, device=dev, dtype=torch.bool)
+    prev_reach = (vr.states.view(S, N, -1)[:, :n, :pd] - vr.goals.view(S, n, -1)[:, :, :pd]).norm(dim=2) < d2g
+    final = vr.states.view(S, N, -1).clone()
+    per_env_reward = torch.vmap(env._reward)                 # the env's own reward, one episode per batch entry
+    live = np.arange(S)
+
+    def policy(batch):
+        return algo.apply_batch(batch, rand=rand, max_iter=max_iter)
+
+    while live.size:
+        out = vr.step(store=False, policy=policy)
+        L = live.size
+        r = per_env_reward(out['action'].view(L, n, -1), out['reach'], prev_reach, out['collision'])      # [L, n]
+        li = torch.from_numpy(live).to(dev)
+        reward.index_add_(0, li, r.to(torch.float64).mean(dim=1))
+        safe[li] = safe[li] & ~out['collision']
+        reach[li] = out['reach']
+        length[live] += 1
+        prev_reach = out['reach']
+        done = (vr.t >= max_steps) | out['reach'].all(dim=1).cpu().numpy()
+        if done.any():
+            ended = np.nonzero(done)[0]
+            final[torch.from_numpy(live[ended]).to(dev)] = vr.states.view(L, N, -1)[torch.from_numpy(ended).to(dev)]
+            stay = np.nonzero(~done)[0]
+            if stay.size:
+                vr.keep(stay)
+                prev_reach = prev_reach[torch.from_numpy(stay).to(dev)]
+            live = live[stay]
+    frac = lambda m: m.sum(dim=1).cpu().numpy() / n           # noqa: E731  (agent counts / n, as eval_ctrl_epi divides)
+    res = {'reward': reward.cpu().numpy(), 'length': length, 'safe': frac(safe), 'reach': frac(reach), 'success': frac(safe & reach)}
+    stats = list(res.items())
+    res['mean'] = {k: float(np.mean(v)) for k, v in stats}
+    res['std'] = {k: float(np.std(v)) for k, v in stats}
+    res['final_states'] = final.cpu()
+    res['seeds'] = seeds
+    return res

@@ -30,16 +30,16 @@ class _StepFunction(torch.autograd.Function):
     """x+ = x + dt f(x, clamp(u + u_ref(x))): forward_graph's state update with its VJP to the action."""
 
     @staticmethod
-    def forward(ctx, states, action, env, num_graphs, freeze):
+    def forward(ctx, states, action, env, num_graphs, freeze, goal_per_graph=None):
         _C.require_cuda(states, action)
         st, ld = ops._mat(states)
         act = action.detach().contiguous()
         cfg = env._cfg(num_graphs)
         nxt = torch.empty(st.shape[0], ld, device=st.device, dtype=torch.float32)
         pass_mask = torch.empty(act.shape, device=st.device, dtype=torch.uint8)
-        goal, ldg = ops._mat(env._goal)
-        _C.call('gcbf_step_fwd', ctypes.byref(cfg), _C.ptr(st), ld, _C.ptr(act), _C.ptr(goal), ldg, _C.ptr(env._gain()),
-                1 if freeze else 0, _C.ptr(nxt), _C.ptr(pass_mask))
+        goal, ldg = ops._mat(env._goal if goal_per_graph is None else goal_per_graph.contiguous())
+        _C.call('gcbf_step_fwd' if goal_per_graph is None else 'gcbf_step_fwd_multi', ctypes.byref(cfg), _C.ptr(st), ld, _C.ptr(act),
+                _C.ptr(goal), ldg, _C.ptr(env._gain()), 1 if freeze else 0, _C.ptr(nxt), _C.ptr(pass_mask))
         ctx.env, ctx.num_graphs, ctx.ld = env, num_graphs, ld
         ctx.save_for_backward(pass_mask)
         return nxt[:, :st.shape[1]] if ld != st.shape[1] else nxt
@@ -51,7 +51,7 @@ class _StepFunction(torch.autograd.Function):
         cfg = ctx.env._cfg(ctx.num_graphs)
         d_action = torch.empty(pass_mask.shape, device=dn.device, dtype=torch.float32)
         _C.call('gcbf_step_bwd', ctypes.byref(cfg), _C.ptr(dn), ld, _C.ptr(pass_mask), _C.ptr(d_action))
-        return None, d_action, None, None, None
+        return None, d_action, None, None, None, None
 
 
 class MultiAgentEnv(ABC):
@@ -197,9 +197,12 @@ class MultiAgentEnv(ABC):
         (gcbf/algo/gcbf.py:195-199): every graph is a *single* graph there, so the reach-freeze branch applies."""
         return _StepFunction.apply(data.states, action, self, self._num_graphs_of(data), True)
 
-    def forward_graph(self, data, action: Tensor):
-        """Graph after one step with RETAINED edges and recomputed edge features (differentiable w.r.t. action)."""
-        state = self.next_states(data, action)
+    def forward_graph(self, data, action: Tensor, single: bool = False, goal: Optional[Tensor] = None):
+        """Graph after one step with RETAINED edges and recomputed edge features (differentiable w.r.t. action).  single: every graph
+        of the batch is a single graph of the reference (reach-freeze branch per graph, as the test-time controller needs);
+        goal [B * n, goal_dim]: one goal set per graph instead of env._goal."""
+        B = self._num_graphs_of(data)
+        state = _StepFunction.apply(data.states, action, self, B, single or B == 1, goal)     # = next_states by default
         fields = dict(x=data.x, edge_index=data.edge_index, edge_attr=self.edge_attr(state, data.edge_index),
                       pos=state[:, :self.POS_DIM], states=state)
         if hasattr(data, 'agent_mask'):

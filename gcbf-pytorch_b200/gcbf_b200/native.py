@@ -94,6 +94,9 @@ SIGS = {
     'gcbf_step_backward': (c_int, [POINTER(StepDesc), POINTER(StepBatch), POINTER(StepCtx), POINTER(StepOut), POINTER(c_void_p), P, P]),
     'gcbf_apply_workspace_bytes': (c_size_t, [POINTER(StepDesc), POINTER(StepBatch)]),
     'gcbf_apply': (c_int, [POINTER(StepDesc), POINTER(StepBatch), c_float, c_float, P, c_int, P, c_int, POINTER(c_int), P, c_size_t, P]),
+    'gcbf_apply_batch_workspace_bytes': (c_size_t, [POINTER(StepDesc), POINTER(StepBatch)]),
+    'gcbf_apply_batch': (c_int, [POINTER(StepDesc), POINTER(StepBatch), c_float, c_float, P, c_int, P, c_int, P, POINTER(c_int), P, c_size_t,
+                                 P]),
     'gcbf_linear_fwd_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P]),
     'gcbf_linear_bwd_data_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
                                        c_int, c_int, c_int, P]),

@@ -436,6 +436,20 @@ int gcbf_step_backward(const gcbf_step_desc* d, const gcbf_step_batch* b, gcbf_s
 size_t gcbf_apply_workspace_bytes(const gcbf_step_desc* d, const gcbf_step_batch* graph);
 int gcbf_apply(const gcbf_step_desc* d, const gcbf_step_batch* graph, float lr, float rand, const float* noise, int max_iter,
                float* action, int ld_action, int* iterations, void* workspace, size_t workspace_bytes, void* stream);
+/* The same controller for d->env.num_graphs graphs of nodes_per_graph nodes each (agents first, edges inside the graphs, as the
+ * radius-graph kernels make them) in one call: many evaluation episodes step at once.  Goals are shared, or one set per graph with
+ * d->goal_per_graph.  noise [(max_iter + 1), num_agents_total, action_dim]: round k of graph g reads rows g*n .. g*n+n-1 of slice k,
+ * so concatenated per-graph draws reproduce per-graph calls.  Per graph g the result is gcbf_apply on graph g alone: the mean in
+ * the loss runs over g's n agents, Adam runs per agent, and g is done at the first round where none of its agents violates or the
+ * round counter passed max_iter; from then on nothing of g changes (no Adam step, no noise, its flags are not re-evaluated), while
+ * its rows keep going through the passes until the slowest graph is done.  rounds (device int32[num_graphs], required) = the Adam
+ * rounds each graph did (gcbf_apply's *iterations for that graph); *iterations (host, optional) = those of the slowest graph.  Still
+ * one host sync per round (the number of graphs still refining).  Spectral norm: the CBF passes run in the order of a single call
+ * (h, actor, nominal h_next, one per round) and power iteration depends on the weights alone, so pass k uses the sigma of pass k
+ * of a single call, and afterwards the CBF's u, v are those a single call on the slowest graph leaves. */
+size_t gcbf_apply_batch_workspace_bytes(const gcbf_step_desc* d, const gcbf_step_batch* batch);
+int gcbf_apply_batch(const gcbf_step_desc* d, const gcbf_step_batch* batch, float lr, float rand, const float* noise, int max_iter,
+                     float* action, int ld_action, int32_t* rounds, int* iterations, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * MACBF, the paper's baseline algorithm (gcbf/algo/macbf.py:20-239; SURVEY 8f-4): the kernels it needs beyond the ones above.
