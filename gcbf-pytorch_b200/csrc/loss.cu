@@ -19,7 +19,7 @@ __global__ void loss_partials_kernel(const float* __restrict__ h, const float* _
                                      const float* __restrict__ hnn, const float* __restrict__ act, int ad,
                                      const uint8_t* __restrict__ safe, const uint8_t* __restrict__ unsafe, int64_t M,
                                      float alpha, float eps, float dt, double* __restrict__ partial,
-                                     float* __restrict__ hdot_out) {
+                                     float* __restrict__ hdot_out, const float* __restrict__ hdot_in) {
   double acc[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
     const float hi = h[i];
@@ -33,7 +33,8 @@ __global__ void loss_partials_kernel(const float* __restrict__ h, const float* _
       acc[GCBF_LP_CNT_SAFE] += 1.0;
       acc[GCBF_LP_OK_SAFE] += (hi >= 0.f) ? 1.0 : 0.0;
     }
-    const float hd = hdot_value(hi, hn[i], hnn[i], dt);  // gcbf.py:207
+    // gcbf.py:207; hdot_in: the analytic h_dot (GCBF.params['h_dot'] = 'analytic') instead of the finite difference
+    const float hd = hdot_in ? hdot_in[i] : hdot_value(hi, hn[i], hnn[i], dt);
     if (hdot_out) hdot_out[i] = hd;
     acc[GCBF_LP_SUM_HDOT] += fmaxf(__fadd_rn(__fsub_rn(-hd, __fmul_rn(alpha, hi)), eps), 0.f);
     acc[GCBF_LP_CNT_ALL] += 1.0;
@@ -61,7 +62,8 @@ __global__ void loss_grads_kernel(const float* __restrict__ h, const float* __re
                                   const uint8_t* __restrict__ safe, const uint8_t* __restrict__ unsafe, int64_t M,
                                   float alpha, float eps, float dt, float cu, float cs, float ch, float ca,
                                   const double* __restrict__ partial, float* __restrict__ d_h,
-                                  float* __restrict__ d_hn, float* __restrict__ d_act, float* __restrict__ scalars) {
+                                  float* __restrict__ d_hn, float* __restrict__ d_act, float* __restrict__ scalars,
+                                  const float* __restrict__ hdot_in, float* __restrict__ d_hdot) {
   const double cnt_u = partial[GCBF_LP_CNT_UNSAFE], cnt_s = partial[GCBF_LP_CNT_SAFE], cnt = partial[GCBF_LP_CNT_ALL];
   const float inv_u = cnt_u > 0 ? (float)(1.0 / cnt_u) : 0.f;
   const float inv_s = cnt_s > 0 ? (float)(1.0 / cnt_s) : 0.f;
@@ -83,10 +85,15 @@ __global__ void loss_grads_kernel(const float* __restrict__ h, const float* __re
   float g = 0.f;
   if (unsafe[i] && __fadd_rn(hi, eps) > 0.f) g += cu * inv_u;
   if (safe[i] && __fadd_rn(-hi, eps) > 0.f) g -= cs * inv_s;
-  const float hd = hdot_value(hi, hn[i], hnn[i], dt);
+  const float hd = hdot_in ? hdot_in[i] : hdot_value(hi, hn[i], hnn[i], dt);
   const bool on = __fadd_rn(__fsub_rn(-hd, __fmul_rn(alpha, hi)), eps) > 0.f;
   float gn = 0.f;
-  if (on) {
+  if (hdot_in) {
+    // analytic h_dot: d/dh of relu(-h_dot - alpha*h + eps) = -alpha ; d/dh_dot = -1
+    const float w = on ? ch * inv_m : 0.f;
+    g -= w * alpha;
+    d_hdot[i] = -w;
+  } else if (on) {
     const float w = ch * inv_m;
     // d/dh of relu(-(h_next - h)/dt - alpha*h + eps) = +1/dt - alpha ; d/dh_next = -1/dt   (the re-linked
     // h_next_new enters only through the detached residue)
@@ -94,7 +101,7 @@ __global__ void loss_grads_kernel(const float* __restrict__ h, const float* __re
     gn = -(w / dt);
   }
   d_h[i] = g;
-  d_hn[i] = gn;
+  if (d_hn) d_hn[i] = gn;
   for (int k = 0; k < ad; ++k) d_act[i * ad + k] = ca * inv_m * 2.f * act[i * ad + k];
 }
 
@@ -142,7 +149,7 @@ extern "C" int gcbf_loss_partials(const float* h, const float* h_next, const flo
   GCBF_REQUIRE(h && h_next && h_next_new && action && safe && unsafe, "gcbf_loss_partials: null pointer");
   const int grid = (int)imin64(ceil_div(M, 256), 4 * kNumSMs);
   loss_partials_kernel<<<grid, 256, 0, st>>>(h, h_next, h_next_new, action, action_dim, safe, unsafe, M, alpha, eps, dt,
-                                            partial, hdot_out);
+                                            partial, hdot_out, nullptr);
   GCBF_LAUNCH_OK();
   return GCBF_OK;
 }
@@ -157,7 +164,35 @@ extern "C" int gcbf_loss_grads(const float* h, const float* h_next, const float*
                "gcbf_loss_grads: null pointer");
   loss_grads_kernel<<<max(1, ceil_div(M, 256)), 256, 0, as_stream(stream)>>>(
       h, h_next, h_next_new, action, action_dim, safe, unsafe, M, alpha, eps, dt, coef_unsafe, coef_safe, coef_hdot,
-      coef_action, partial, d_h, d_h_next, d_action, scalars);
+      coef_action, partial, d_h, d_h_next, d_action, scalars, nullptr, nullptr);
+  GCBF_LAUNCH_OK();
+  return GCBF_OK;
+}
+
+// the same two passes with the analytic h_dot as an input (GCBF.params['h_dot'] = 'analytic'): same partial layout, scalars and masked
+// means; d_hdot replaces d_h_next
+extern "C" int gcbf_loss_partials_hdot(const float* h, const float* hdot, const float* action, int action_dim, const uint8_t* safe,
+                                       const uint8_t* unsafe, int64_t M, float alpha, float eps, double* partial, void* stream) {
+  GCBF_REQUIRE(partial && M >= 0 && action_dim >= 0, "gcbf_loss_partials_hdot: bad arguments");
+  if (M > 0) GCBF_REQUIRE(h && hdot && action && safe && unsafe, "gcbf_loss_partials_hdot: null pointer");
+  cudaStream_t st = as_stream(stream);
+  GCBF_CUDA_OK(cudaMemsetAsync(partial, 0, GCBF_LP_SIZE * sizeof(double), st));
+  if (M == 0) return GCBF_OK;
+  const int grid = (int)imin64(ceil_div(M, 256), 4 * kNumSMs);
+  loss_partials_kernel<<<grid, 256, 0, st>>>(h, nullptr, nullptr, action, action_dim, safe, unsafe, M, alpha, eps, 1.f, partial, nullptr, hdot);
+  GCBF_LAUNCH_OK();
+  return GCBF_OK;
+}
+
+extern "C" int gcbf_loss_grads_hdot(const float* h, const float* hdot, const float* action, int action_dim, const uint8_t* safe,
+                                    const uint8_t* unsafe, int64_t M, float alpha, float eps, float coef_unsafe, float coef_safe,
+                                    float coef_hdot, float coef_action, const double* partial, float* d_h, float* d_hdot, float* d_action,
+                                    float* scalars, void* stream) {
+  GCBF_REQUIRE(partial && scalars && M >= 0 && action_dim >= 0, "gcbf_loss_grads_hdot: bad arguments");
+  GCBF_REQUIRE(M == 0 || (h && hdot && action && safe && unsafe && d_h && d_hdot && d_action), "gcbf_loss_grads_hdot: null pointer");
+  loss_grads_kernel<<<max(1, ceil_div(M, 256)), 256, 0, as_stream(stream)>>>(
+      h, nullptr, nullptr, action, action_dim, safe, unsafe, M, alpha, eps, 1.f, coef_unsafe, coef_safe, coef_hdot, coef_action, partial,
+      d_h, nullptr, d_action, scalars, hdot, d_hdot);
   GCBF_LAUNCH_OK();
   return GCBF_OK;
 }

@@ -89,6 +89,13 @@ _SIGS = {
     'gcbf_state_dot': (c_int, [POINTER(EnvCfg), P, c_int, P, P, P, c_int, c_int, c_int, P, c_int, P]),
     'gcbf_edge_attr_tangent': (c_int, [c_int, P, c_int, P, c_int, P, c_int64, P, P]),
     'gcbf_attn_aggr_tangent': (c_int, [P, c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, P]),
+    # backward of the analytic h_dot pass (csrc/jvp.cu, csrc/loss.cu)
+    'gcbf_attn_aggr_tangent_bwd': (c_int, [P, c_int, P, c_int, P, P, P, c_int, c_int, P, c_int, P, c_int, P, P, c_int, P, c_int, P]),
+    'gcbf_act_tangent_bwd': (c_int, [P, P, P, P, c_int64, c_int, P, P, P]),
+    'gcbf_state_dot_bwd': (c_int, [POINTER(EnvCfg), P, c_int, P, P, P, c_int, c_int, c_int, P, c_int, P, c_int, P]),
+    'gcbf_edge_attr_bwd_ordered': (c_int, [c_int, P, c_int, P, c_int64, c_int, P, P, P]),
+    'gcbf_loss_partials_hdot': (c_int, [P, P, P, c_int, P, P, c_int64, c_float, c_float, P, P]),
+    'gcbf_loss_grads_hdot': (c_int, [P, P, P, c_int, P, P, c_int64, c_float, c_float, c_float, c_float, c_float, c_float, P, P, P, P, P, P]),
     'gcbf_macbf_loss_grads': (c_int, [P, P, P, P, c_int64, P, c_int, c_int64, c_float, c_float, c_float, c_float, c_float, c_float,
                                       c_float, P, P, P, P, P, P]),
 }

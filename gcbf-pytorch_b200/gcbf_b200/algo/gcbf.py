@@ -167,7 +167,11 @@ class GCBF(Algorithm):
         """One inner iteration of GCBF.update (gcbf.py:158-226) on a collated batch.  Returns device tensors
         (no host sync): 'scalars' = [loss_unsafe, loss_safe, loss_h_dot, loss_action, acc_unsafe, acc_safe,
         total_loss, num_agents], 'acc_h_dot', plus h / actions / h_next / h_next_new for inspection (views into the step's
-        workspace: valid until the next train_step of this object)."""
+        workspace: valid until the next train_step of this object).
+        params['h_dot'] selects the CBF-condition loss: 'finite_difference' (the default, the reference's) or 'analytic'
+        (_train_step_analytic)."""
+        if self._h_dot_mode() == 'analytic':
+            return self._train_step_analytic(graphs, apply_optim, compute_acc_h_dot)
         if ops.NATIVE:
             return self._train_step_native(graphs, apply_optim, compute_acc_h_dot)
         from ..arena import ARENA
@@ -176,6 +180,64 @@ class GCBF(Algorithm):
             return self._train_step(graphs, apply_optim, compute_acc_h_dot)
         finally:
             ARENA.end()
+
+    H_DOT_MODES = ('finite_difference', 'analytic')
+
+    def _h_dot_mode(self) -> str:
+        mode = self.params.get('h_dot', 'finite_difference')
+        if mode not in self.H_DOT_MODES:
+            raise ValueError(f"params['h_dot'] must be one of {self.H_DOT_MODES}, got {mode!r}")
+        return mode
+
+    def _train_step_analytic(self, graphs, apply_optim: bool, compute_acc_h_dot: bool) -> Dict[str, Tensor]:
+        """One inner iteration with the analytic h_dot in the CBF-condition loss (params['h_dot'] = 'analytic'): the losses, masked
+        means and accuracies of gcbf.py:164-218 with h_dot = J_h(s) . f(s, clamp(actions + u_ref(s))) (gcbf_b200/jvp.py: the edges
+        of `graphs` held fixed, the same 1/sigma and u, v as h -- ONE power iteration, where the finite-difference step does three) in
+        place of the finite difference, differentiated through: the CBF gets gradients through h and h_dot (incl. the second-order
+        terms of the attention softmax, the head's tanh and sigma), the actor through loss_action and h_dot -> x_dot -> clamp -> actions.
+        No h_next, no re-linked graph.  Python-sequenced on the current stream."""
+        from .. import jvp
+        env, hp = self._env, self.params
+        bucket = self._ensure_bucket()
+        dev = graphs.states.device
+        red = self._reducer()
+        M = graphs.u_ref.shape[0]
+        a_dim = self.action_dim
+
+        h, state = jvp.cbf_forward_saved(self.cbf, graphs)               # gcbf.py:161  (the one power iteration)
+        actions = self.actor(graphs)                                     # gcbf.py:162
+        masks = env._masks(graphs)                                       # gcbf.py:168, 180
+        actd = actions.detach()
+        hdot = jvp.h_dot_tangent(env, graphs, actd, state, keep=True)    # [M, 1]
+
+        partial = torch.empty(16, device=dev, dtype=torch.float64)
+        safe_u8, unsafe_u8 = masks[0].view(torch.uint8), masks[1].view(torch.uint8)
+        _C.call('gcbf_loss_partials_hdot', _C.ptr(h), _C.ptr(hdot), _C.ptr(actd), a_dim, _C.ptr(safe_u8), _C.ptr(unsafe_u8), M,
+                float(hp['alpha']), float(hp['eps']), _C.ptr(partial))
+        red.sum_(partial)                                                # global counts => global masked means
+        d_h, d_hdot, d_act = torch.empty_like(h), torch.empty_like(hdot), torch.empty_like(actd)
+        scalars = torch.empty(8, device=dev, dtype=torch.float32)
+        _C.call('gcbf_loss_grads_hdot', _C.ptr(h), _C.ptr(hdot), _C.ptr(actd), a_dim, _C.ptr(safe_u8), _C.ptr(unsafe_u8), M,
+                float(hp['alpha']), float(hp['eps']), float(hp['loss_unsafe_coef']), float(hp['loss_safe_coef']),
+                float(hp['loss_h_dot_coef']), float(hp['loss_action_coef']), _C.ptr(partial), _C.ptr(d_h), _C.ptr(d_hdot),
+                _C.ptr(d_act), _C.ptr(scalars))
+
+        bucket.zero_grad()
+        ops.GRAD_INTO_PARAM = True     # weight-grad kernels accumulate straight into the bucket's .grad views
+        try:
+            jvp.cbf_backward(env, graphs, actd, state, d_h, d_hdot, d_act)   # CBF gradients; d_act += the h_dot path
+            torch.autograd.backward(actions, d_act)
+        finally:
+            ops.GRAD_INTO_PARAM = False
+
+        hdot = hdot.reshape(-1)
+        out = dict(scalars=scalars, h=h, actions=actd.clone(), safe_mask=masks[0], unsafe_mask=masks[1], hdot=hdot)
+        if compute_acc_h_dot:                                            # gcbf.py:209 (M x M broadcast mean)
+            out['acc_h_dot'] = self._acc_h_dot(red, hdot, h, M, dev)
+        red.sum_(bucket.grad)                                            # the ONE gradient collective
+        if apply_optim:
+            self.optim_step()
+        return out
 
     def _train_step(self, graphs, apply_optim: bool, compute_acc_h_dot: bool) -> Dict[str, Tensor]:
         env, hp = self._env, self.params
@@ -597,7 +659,7 @@ class GCBF(Algorithm):
             self.last_apply_batch_rounds = graph_rounds.cpu().to(torch.int64)
         return action
 
-    # ---- analytic h_dot (SURVEY section 8f-3; additive: the training loss keeps the reference's finite difference) ------------------
+    # ---- analytic h_dot (SURVEY section 8f-3; the training loss uses it when params['h_dot'] = 'analytic') --------------------------
     def h_dot_analytic(self, data, action: Optional[Tensor] = None, freeze: Optional[bool] = None):
         """(h, h_dot) with h_dot_i = sum_k dh_i/ds_k . f(s_k, clamp(u_k + u_ref)) as one forward-mode pass (gcbf_b200/jvp.py): the
         derivative the finite difference (h(x + dt f) - h(x)) / dt of gcbf.py:193-207 approximates, edges held fixed.  action: the

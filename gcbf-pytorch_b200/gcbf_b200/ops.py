@@ -729,19 +729,25 @@ def _grad_targets(L):
 
 def mlp_backward(ctx: MLPCtx, layers: Sequence[LinearSpec], dy: torch.Tensor, need_dx: bool,
                  dx_out: Optional[torch.Tensor] = None, dx_accumulate: bool = False, dy_amax: Optional[torch.Tensor] = None,
-                 dx_amax: Optional[torch.Tensor] = None):
+                 dx_amax: Optional[torch.Tensor] = None, mask_acts: Optional[List[torch.Tensor]] = None, bias_grad: bool = True,
+                 dy_is_preact: bool = False):
     """Returns (dx or None, [(dW, db) per layer]).  `dy_amax`: amax slot of dy when its producer reduced it (only valid if
     the output layer has no activation).  `dx_amax`: slot that receives max|dx| when the input-gradient GEMM runs on the
-    tensor cores (the caller checks `dx_amax_valid`)."""
+    tensor cores (the caller checks `dx_amax_valid`).
+    The backward of a tangent pass (gcbf_b200/jvp.py) runs this on the tangent's layer inputs (ctx.acts) with: `mask_acts` the
+    PRIMAL activations the hidden ReLU masks come from, `bias_grad=False` (the tangent layers have no bias) and `dy_is_preact`
+    (dy is already the gradient of the output layer's pre-activation)."""
     grads = [None] * len(layers)
     dz = dy
     last = len(layers) - 1
-    if layers[last].act == ACT_TANH:
+    if dy_is_preact:
+        pass
+    elif layers[last].act == ACT_TANH:
         dz = act_bwd(dz, ctx.acts[last + 1], ACT_TANH)
     elif layers[last].act == ACT_RELU:
         dz = act_bwd(dz, ctx.acts[last + 1], ACT_RELU)
     # amax of dz when the producing data-grad epilogue already reduced it
-    dz_amax = dy_amax if layers[last].act == ACT_NONE else None
+    dz_amax = dy_amax if (dy_is_preact or layers[last].act == ACT_NONE) else None
     mlp_backward.dx_amax_valid = False
     for l in range(last, -1, -1):
         L = layers[l]
@@ -753,7 +759,9 @@ def mlp_backward(ctx: MLPCtx, layers: Sequence[LinearSpec], dy: torch.Tensor, ne
             # one fp16 companion of dz serves the weight-grad (MN-major A) and the data-grad (K-major A); the bias
             # gradient (column sums of dz) is fused into the split
             gW, gb = (None, None) if SKIP_WGRAD else _grad_targets(L)
-            db = None if SKIP_WGRAD else (gb if gb is not None else _empty(N, device=dz.device, dtype=torch.float32))
+            if not bias_grad:
+                gb = None
+            db = None if (SKIP_WGRAD or not bias_grad) else (gb if gb is not None else _empty(N, device=dz.device, dtype=torch.float32))
             dzh = split_h(dz, amax=dz_amax, colsum=db, colsum_accumulate=gb is not None)
             if SKIP_WGRAD:
                 grads[l] = (None, None)
@@ -771,7 +779,7 @@ def mlp_backward(ctx: MLPCtx, layers: Sequence[LinearSpec], dy: torch.Tensor, ne
                 assert layers[l - 1].act == ACT_RELU
                 Kp = ctx.acts[l - 1].shape[1]
                 dz_amax = amax_slot(dz.device) if use_h(M, K, Kp) else None
-                dz = linear_bwd_data_h(dzh, wh, inv_sigma, x_in, out_amax=dz_amax)
+                dz = linear_bwd_data_h(dzh, wh, inv_sigma, x_in if mask_acts is None else mask_acts[l], out_amax=dz_amax)
             elif need_dx:
                 dz = linear_bwd_data_h(dzh, wh, inv_sigma, None, out=dx_out, accumulate=dx_accumulate, out_amax=dx_amax)
                 mlp_backward.dx_amax_valid = dx_amax is not None
@@ -783,19 +791,21 @@ def mlp_backward(ctx: MLPCtx, layers: Sequence[LinearSpec], dy: torch.Tensor, ne
             grads[l] = (None, None)
         else:
             gW, gb = _grad_targets(L)
+            if not bias_grad:
+                gb = None
             if L.sn:
-                dW, db = linear_bwd_weight(dz, x_in, inv_sigma)
+                dW, db = linear_bwd_weight(dz, x_in, inv_sigma, need_bias=bias_grad)
                 u, v = ctx.uv[l]
                 sn_grad_fixup(dW, L.W, u, v, inv_sigma, acc=gW)
                 if gb is not None:
                     gb.add_(db)
             else:
-                dW, db = linear_bwd_weight(dz, x_in, inv_sigma, out_w=gW, out_b=gb)
+                dW, db = linear_bwd_weight(dz, x_in, inv_sigma, need_bias=bias_grad, out_w=gW, out_b=gb)
             grads[l] = (None if gW is not None else dW, None if gb is not None else db)
         if l > 0:
             # hidden ReLU of layer l-1 folded into the epilogue: dz_{l-1} = (dz_l W_l) * (y_{l-1} > 0)
             assert layers[l - 1].act == ACT_RELU
-            dz = linear_bwd_data(dz, L.W, inv_sigma, x_in)
+            dz = linear_bwd_data(dz, L.W, inv_sigma, x_in if mask_acts is None else mask_acts[l])
         elif need_dx:
             dz = linear_bwd_data(dz, L.W, inv_sigma, None, out=dx_out, accumulate=dx_accumulate)
         else:

@@ -493,8 +493,8 @@ int gcbf_macbf_loss_grads(const float* h, const float* h_next, const uint8_t* sa
                           float* d_h_next, float* d_action, float* scalars, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
- * Analytic h_dot (SURVEY 8f-3; an ADDITIVE alternative to the finite difference of gcbf/algo/gcbf.py:193-207, not used by the
- * training loss): h_dot_i = sum_k (dh_i/ds_k) . f(s_k, u_k) with the edges held fixed, as a forward-mode pass.  The linear layers
+ * Analytic h_dot (SURVEY 8f-3; an ADDITIVE alternative to the finite difference of gcbf/algo/gcbf.py:193-207, which the training
+ * loss uses by default; the backward entry points below train through it): h_dot_i = sum_k (dh_i/ds_k) . f(s_k, u_k) with the edges held fixed, as a forward-mode pass.  The linear layers
  * of the tangent reuse gcbf_linear_fwd* (no bias, no activation) and gcbf_act_bwd (activation derivative); the other pieces:
  *   gcbf_state_dot         x_dot = f(x, clamp(action + u_ref)) for every node (dynamics of simple_car.py:78-89, dubins_car.py:110-132,
  *                          simple_drone.py:103-120; u_ref [num_graphs * num_agents, a] from gcbf_u_ref; freeze != 0: the single-graph
@@ -508,6 +508,45 @@ int gcbf_edge_attr_tangent(int env, const float* states, int ld_state, const flo
                            int64_t num_edges, float* t_edge_attr, void* stream);
 int gcbf_attn_aggr_tangent(const float* msg, int ld_msg, const float* t_msg, int ld_tmsg, const float* att, const float* t_gate,
                            const int32_t* rowptr, int num_nodes, int channels, float* t_aggr, int ld_taggr, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------
+ * Backward of the analytic h_dot pass: the opt-in CBF-condition loss of GCBF.params['h_dot'] = 'analytic', which trains through
+ * h_dot = J_h(s) . f(s, clamp(u + u_ref)) instead of the finite difference of gcbf/algo/gcbf.py:193-207.  Deterministic, no float atomics.
+ *   gcbf_attn_aggr_tangent_bwd  VJP of gcbf_attn_aggr_tangent.  With tau = d L / d t_aggr_i, p_e = msg_e . tau, q_e = t_msg_e . tau,
+ *                               gbar_i = sum_k a_k t_gate_k, P_i = sum_k a_k p_k:  d_t_msg_e = a_e tau,  d_t_gate_e = a_e (p_e - P_i), and the
+ *                               second-order terms  d_msg_e += a_e (t_gate_e - gbar_i) tau,  d_gate_e += a_e (r_e - sum_k a_k r_k) with
+ *                               r_e = q_e + t_gate_e (p_e - P_i) - gbar_i p_e, added onto the primal gcbf_attn_aggr_bwd gradients
+ *                               (accumulate = 0: written).  One warp per target; any channel count and pitch.  The edge arrays may be
+ *                               null when the batch has no edges.
+ *   gcbf_act_tangent_bwd        element-wise, y = act(z), y_dot = act'(z) z_dot:  ReLU  dZ = [Y > 0] dY, dTZ = [Y > 0] dTY;  tanh  dTZ =
+ *                               (1 - Y^2) dTY, dZ = (1 - Y^2)(dY - 2 Y TZ dTY) (TZ: the pre-activation tangent z_dot, read for tanh only);
+ *                               none  identity.
+ *   gcbf_state_dot_bwd          d L / d action [num_graphs * num_agents, a] from d L / d x_dot [nodes, >= state_dim]: the VJP of gcbf_state_dot
+ *                               (same arguments) through the clamp (gradient passes where -lim <= action + u_ref <= lim, as torch.clamp) and
+ *                               the reach-freeze (zero for frozen agents); obstacle rows carry no action.  accumulate: add onto d_action.
+ *   gcbf_edge_attr_bwd_ordered  d states += d edge_attr . d edge_attr / d states (the VJP of gcbf_edge_attr_fwd, equal to gcbf_edge_attr_bwd
+ *                               to rounding) summed in a fixed order per node: bit-reproducible.  d_states has pitch ld_state and is
+ *                               accumulated into.  PRECONDITION: edge_index[1] (targets) sorted ascending, as every graph this library
+ *                               builds is (each node's target-side run is found by binary search; unsorted edges give wrong gradients).  Since the edge tangent is linear in s_dot with the same Jacobian, this is also its VJP.
+ *   gcbf_loss_partials_hdot /   gcbf_loss_partials / gcbf_loss_grads with h_dot an input: same partial layout, scalars and masked means;
+ *   gcbf_loss_grads_hdot        d_hdot = d loss / d h_dot takes the place of d_h_next.
+ * ------------------------------------------------------------------------------------------------- */
+int gcbf_attn_aggr_tangent_bwd(const float* msg, int ld_msg, const float* t_msg, int ld_tmsg, const float* att, const float* t_gate,
+                               const int32_t* rowptr, int num_nodes, int channels, const float* d_t_aggr, int ld_dtaggr, float* d_t_msg,
+                               int ld_dtmsg, float* d_t_gate, float* d_msg, int ld_dmsg, float* d_gate, int accumulate, void* stream);
+int gcbf_act_tangent_bwd(const float* dY, const float* dTY, const float* Y, const float* TZ, int64_t count, int act, float* dZ, float* dTZ,
+                         void* stream);
+int gcbf_state_dot_bwd(const gcbf_env_cfg* cfg, const float* states, int ld_state, const float* action, const float* u_ref,
+                       const float* goal, int ld_goal, int goal_per_graph, int freeze, const float* d_state_dot, int ld_dsdot,
+                       float* d_action, int accumulate, void* stream);
+int gcbf_edge_attr_bwd_ordered(int env, const float* states, int ld_state, const int64_t* edge_index, int64_t num_edges, int num_nodes,
+                               const float* d_edge_attr, float* d_states, void* stream);
+int gcbf_loss_partials_hdot(const float* h, const float* hdot, const float* action, int action_dim, const uint8_t* safe,
+                            const uint8_t* unsafe, int64_t num_agents_total, float alpha, float eps, double* partial, void* stream);
+int gcbf_loss_grads_hdot(const float* h, const float* hdot, const float* action, int action_dim, const uint8_t* safe,
+                         const uint8_t* unsafe, int64_t num_agents_total, float alpha, float eps, float coef_unsafe, float coef_safe,
+                         float coef_hdot, float coef_action, const double* partial, float* d_h, float* d_hdot, float* d_action,
+                         float* scalars, void* stream);
 
 /* instrumentation (bench.py): kernels launched by the chain-level calls since the last reset, and optional CUDA-event timing of
  * every linear-layer launch (kind 0 forward / 1 data-grad / 2 weight-grad on the tensor cores, 3 fp32 linear kernels, 4 operand
