@@ -76,11 +76,15 @@ bool timing_on();      // per-launch CUDA-event timing enabled (gcbf_timing_enab
 int check_net(const gcbf_net_desc* net);
 int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* edge_attr, const int64_t* edge_index,
                 const int32_t* rowptr, int64_t E, int Nn, const int64_t* row_index, int rows, const float* head_extra, float* out,
-                int ld_out, NetCtx* ctx);
+                int ld_out, NetCtx* ctx, const float* const* inv_sigma_in = nullptr);   // inv_sigma_in: skip the power iteration, use these
 int net_backward(Run& R, const gcbf_net_desc& net, const NetCtx& ctx, const int32_t* rowptr, const int64_t* row_index,
                  const float* d_out, int ld_dout, float* d_edge_attr, bool skip_wgrad, cudaEvent_t gamma_done = nullptr);
 int check_step(const gcbf_step_desc* d, const gcbf_step_batch* b, const char* what);   // step.cu
 int vec_add(Run& R, float* dst, const float* src, int64_t n);
+int collect_layers(const gcbf_net_desc& net, const gcbf_linear_desc** all);      // phi, gate, gamma, head in that order
+int sn_power_iter(Run& R, const gcbf_linear_desc* const* layers, int n, bool snapshot, const float** inv_sigma, const float** us,
+                  const float** vs);
+int refresh_weight_companions(Run& R, const gcbf_linear_desc* const* layers, int n);
 size_t net_fwd_bytes(const gcbf_net_desc& net, int64_t E, int Nn, int rows, bool has_row_index, bool save);
 size_t net_bwd_bytes(const gcbf_net_desc& net, int64_t E, int Nn, int rows, bool has_row_index, bool need_d_edge_attr, bool skip_wgrad);
 

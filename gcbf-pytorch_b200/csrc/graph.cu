@@ -9,27 +9,14 @@
 //   metric 1 (DubinsCar / SimpleDrone, gcbf/env/dubins_car.py:730-746, simple_drone.py:316-333):
 //       torch.norm on CPU accumulates acc = fma(d, d, acc) per dim, then sqrt (measured against torch
 //       2.11 CPU: 0 mismatches in 4e6 pairs);  hit = sqrtf(acc) < r, diagonal excluded.
+// The pair rule and the edge-feature map g(s) live in graph_core.h (shared with the probe graphs of field.cu).
 #include "common.cuh"
+#include "graph_core.h"
 
 namespace gcbf {
 
-__device__ __forceinline__ bool pair_hit(const float* __restrict__ pi, const float* __restrict__ pj, int pos_dim,
-                                         float r, float r2, int metric) {
-  if (metric == 0) {
-    float d2 = 0.f;
-    for (int d = 0; d < pos_dim; ++d) {
-      const float diff = __fsub_rn(pi[d], pj[d]);
-      d2 = __fadd_rn(d2, __fmul_rn(diff, diff));
-    }
-    return d2 < r2;
-  }
-  float acc = 0.f;
-  for (int d = 0; d < pos_dim; ++d) {
-    const float diff = __fsub_rn(pi[d], pj[d]);
-    acc = __fmaf_rn(diff, diff, acc);
-  }
-  return __fsqrt_rn(acc) < r;
-}
+using graph::pair_hit;
+using graph::edge_feat;
 
 template <bool FILL>
 __global__ void radius_graph_kernel(const float* __restrict__ states, int ld, int pos_dim, int num_graphs, int N,
@@ -128,21 +115,6 @@ __global__ void rowptr_kernel(const int64_t* __restrict__ dst, int64_t E, int nu
   for (int64_t e = i; e < E; e += (int64_t)gridDim.x * blockDim.x) {
     const int64_t d = dst[e];
     if (d < 0 || d >= num_nodes || (e + 1 < E && dst[e + 1] < d)) *unsorted_flag = 1;
-  }
-}
-
-// g(s) of the edge features
-template <int ENV>
-__device__ __forceinline__ void edge_feat(const float* __restrict__ s, float* f) {
-  if (ENV == GCBF_ENV_DUBINS_CAR) {
-    // reference gcbf/env/dubins_car.py:724-728: [x, y, theta, v*cos(theta), v*sin(theta)]
-    f[0] = s[0]; f[1] = s[1]; f[2] = s[2];
-    f[3] = __fmul_rn(s[3], cosf(s[2]));
-    f[4] = __fmul_rn(s[3], sinf(s[2]));
-  } else if (ENV == GCBF_ENV_SIMPLE_CAR) {
-    f[0] = s[0]; f[1] = s[1]; f[2] = s[2]; f[3] = s[3];
-  } else {
-    f[0] = s[0]; f[1] = s[1]; f[2] = s[2]; f[3] = s[3]; f[4] = s[4]; f[5] = s[5];
   }
 }
 

@@ -408,7 +408,7 @@ static int check_mlp(const gcbf_linear_desc* layers, int n, const char* what) {
 }
 
 // ---- the GNN pass ------------------------------------------------------------------------------------------------------
-static int collect_layers(const gcbf_net_desc& net, const gcbf_linear_desc** all) {
+int collect_layers(const gcbf_net_desc& net, const gcbf_linear_desc** all) {
   int n = 0;
   for (int i = 0; i < net.n_phi; ++i) all[n++] = &net.phi[i];
   for (int i = 0; i < net.n_gate; ++i) all[n++] = &net.gate[i];
@@ -435,7 +435,7 @@ int check_net(const gcbf_net_desc* net) {
 
 int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* edge_attr, const int64_t* edge_index,
                 const int32_t* rowptr, int64_t E64, int Nn, const int64_t* row_index, int rows, const float* head_extra, float* out,
-                int ld_out, NetCtx* ctx) {
+                int ld_out, NetCtx* ctx, const float* const* inv_sigma_in) {
   const int E = (int)E64;
   const int nd = net.node_dim, C = net.phi_dim, kin = 2 * nd + net.edge_dim;
   const bool save = ctx != nullptr;
@@ -446,7 +446,12 @@ int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* e
   const gcbf_linear_desc* all[4 * GCBF_MAX_MLP_LAYERS];
   const int nall = collect_layers(net, all);
   const float *isg[4 * GCBF_MAX_MLP_LAYERS], *us[4 * GCBF_MAX_MLP_LAYERS], *vs[4 * GCBF_MAX_MLP_LAYERS];
-  if (int rc = sn_power_iter(R, all, nall, save, isg, us, vs)) return rc;
+  if (inv_sigma_in) {
+    // 1/sigma of a power iteration the caller already ran (a forward split into several calls: one iteration for all of them)
+    for (int i = 0; i < nall; ++i) { isg[i] = inv_sigma_in[i]; us[i] = nullptr; vs[i] = nullptr; }
+  } else {
+    if (int rc = sn_power_iter(R, all, nall, save, isg, us, vs)) return rc;
+  }
   if (net.refresh_weights) { if (int rc = refresh_weight_companions(R, all, nall)) return rc; }
   const int o_gate = net.n_phi, o_gamma = o_gate + net.n_gate, o_head = o_gamma + net.n_gamma;
   const float *msg, *gate, *feat;

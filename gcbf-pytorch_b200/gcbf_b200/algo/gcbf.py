@@ -669,6 +669,132 @@ class GCBF(Algorithm):
             action = self.act(data)
         return jvp.cbf_value_and_h_dot(self.cbf, self._env, data, action, freeze)
 
+    # ---- CBF level-set field (the data of plot_cbf.py / plot_cbf_contour, gcbf/trainer/utils.py:226-298) ----------------------------
+    FIELD_MAX_PROBES = 65536            # default probe bound of one chunk
+    FIELD_MAX_EDGES = 262144            # default probe-edge bound of one chunk (7 GB of workspace at C3 with the 2048-wide phi)
+
+    @staticmethod
+    def field_grid(lims, x_dim: int, y_dim: int, n_mesh: int):
+        """The grid axes of plot_cbf_contour (utils.py:259-262): np.linspace over the limits' own dtype (float32 box ->
+        float32 axes), as the reference computes them."""
+        lo, hi = lims
+        val = lambda v: v.cpu() if isinstance(v, Tensor) else v
+        xs = np.linspace(val(lo[x_dim]), val(hi[x_dim]), n_mesh)
+        ys = np.linspace(val(lo[y_dim]), val(hi[y_dim]), n_mesh)
+        return xs, ys
+
+    def cbf_field(self, data, agents=0, x_dim: int = 0, y_dim: int = 1, n_mesh: int = 30, lims=None, relink: bool = False,
+                  max_probes: Optional[int] = None, max_edges: Optional[int] = None):
+        """h of the given agents over an n_mesh x n_mesh grid of state dimensions (x_dim, y_dim), everyone else fixed: what
+        plot_cbf_contour draws (gcbf/trainer/utils.py:259-273), for every graph of `data` (one graph or a Batch of equally sized
+        graphs, e.g. every step of an episode) and every agent in `agents` (an id or a list of ids) in ONE library call.
+
+        Returns (xs [n_mesh], ys [n_mesh], h [B, A, n_mesh, n_mesh]) with h[b, k, i, j] = h of agent agents[k] of graph b at
+        state[x_dim] = xs[j], state[y_dim] = ys[i] (np.meshgrid 'xy' order, as the reference's `H[i, j]`).  xs, ys are the numpy
+        axes of np.linspace over `lims` ((low, high), default env.state_lim); the states get their fp32 roundings.
+        relink=False keeps the given edge_index (the reference's plot); relink=True re-links the moved agent to every node inside
+        the communication radius, as add_communication_links would (neighbours enter and leave as it moves).  Like the reference's
+        single cbf(plot_data) call, a call advances the CBF's spectral-norm vectors by ONE power iteration, however many chunks of
+        at most max_probes probes / max_edges probe edges it runs in (gcbf_cbf_field, csrc/field.cu); one host sync per call.
+        The chunk count and the probe edges go to self.last_field_chunks / self.last_field_edges.  The workspace is sized for the
+        call's largest chunk: at most max_probes probes with at most nodes_per_graph - 1 edges each, and at most max_edges edges."""
+        import ctypes
+        from .. import native
+        d, keep, xs, ys, B, A, T = self._field_desc(data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges)
+        layers = keep[-1]
+        dev = data.states.device
+        need = native.fn('gcbf_cbf_field_workspace_bytes')(ctypes.byref(d))
+        if need == 0:
+            native.check(-1, 'gcbf_cbf_field_workspace_bytes')
+        ws = native.workspace(need, dev)
+        h = torch.empty(T, device=dev, dtype=torch.float32)
+        info = (ctypes.c_int64 * 2)()
+        native.check(native.fn('gcbf_cbf_field')(ctypes.byref(d), h.data_ptr(), info, ws.data_ptr(), ws.numel(), _C.stream()), 'gcbf_cbf_field')
+        native._mark_fresh(layers)
+        self.last_field_chunks, self.last_field_edges = int(info[0]), int(info[1])
+        return xs, ys, h.view(B, A, n_mesh, n_mesh)
+
+    def cbf_field_probe_graph(self, data, agents=0, x_dim: int = 0, y_dim: int = 1, n_mesh: int = 30, lims=None, relink: bool = False):
+        """The probe graphs cbf_field feeds the CBF (gcbf_cbf_field_probe_count / _fill), for inspection: (edge_index [2, E],
+        edge_attr [E, edge_dim]) with target = the probe id t = ((b * A + k) * n_mesh + i) * n_mesh + j (agent agents[k] of graph b at
+        (xs[j], ys[i])) and source = the node id in `data`, sorted (t asc, source asc); edge_attr = g(s_source) - g(s'_t).  Same
+        arguments as cbf_field; the CBF is not evaluated (u, v unchanged).  One host sync (the edge count)."""
+        from .. import native
+        import ctypes
+        d, keep, xs, ys, B, A, T = self._field_desc(data, agents, x_dim, y_dim, n_mesh, lims, relink, None, None)
+        dev = data.states.device
+        rowptr = torch.empty(T + 1, device=dev, dtype=torch.int32)
+        native.check(native.fn('gcbf_cbf_field_probe_count')(ctypes.byref(d), rowptr.data_ptr(), _C.stream()), 'gcbf_cbf_field_probe_count')
+        E = int(rowptr[-1].item())
+        ei = torch.empty(2, E, device=dev, dtype=torch.int64)
+        ea = torch.empty(E, self._env.edge_dim, device=dev, dtype=torch.float32)
+        native.check(native.fn('gcbf_cbf_field_probe_fill')(ctypes.byref(d), rowptr.data_ptr(), ei.data_ptr() if E else None, E,
+                                                            ea.data_ptr() if E else None, _C.stream()), 'gcbf_cbf_field_probe_fill')
+        return ei, ea
+
+    def _field_desc(self, data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges):
+        """Argument checks (all before any launch) and the gcbf_field_desc of a field call: (desc, tensors it points into + the CBF's
+        layer list, xs, ys, B, A, T)."""
+        import ctypes
+        from .. import native
+        from ..nn.gnn import cached_rowptr
+        if not isinstance(self.cbf, CBFGNN):
+            raise NotImplementedError(f'cbf_field needs a per-agent CBF (CBFGNN); {type(self).__name__} has a per-edge CBF')
+        env = self._env
+        n, sd = env.num_agents, env.state_dim
+        ids = [agents] if isinstance(agents, (int, np.integer)) else list(agents)
+        if not ids or any(not isinstance(a, (int, np.integer)) or not 0 <= int(a) < n for a in ids):
+            raise ValueError(f'agents must be ids in [0, {n}), got {agents!r}')
+        ids = [int(a) for a in ids]
+        for name, d in (('x_dim', x_dim), ('y_dim', y_dim)):
+            if not isinstance(d, (int, np.integer)) or not 0 <= int(d) < sd:
+                raise ValueError(f'{name} must be in [0, {sd}), got {d!r}')
+        if x_dim == y_dim:
+            raise ValueError(f'x_dim and y_dim must differ, got {x_dim} twice')
+        if not isinstance(n_mesh, (int, np.integer)) or n_mesh < 2:
+            raise ValueError(f'n_mesh must be an integer >= 2, got {n_mesh!r}')
+        if max_probes is not None and int(max_probes) < 1:
+            raise ValueError(f'max_probes must be >= 1, got {max_probes}')
+        for t in (data.states, data.x) + (() if relink else (data.edge_index,)):
+            if not (isinstance(t, Tensor) and t.is_cuda):
+                raise RuntimeError('cbf_field needs CUDA tensors (states, x[, edge_index]): there is no CPU fallback')
+        B = env._num_graphs_of(data)
+        N = env.nodes_per_graph
+        xs, ys = self.field_grid(env.state_lim if lims is None else lims, int(x_dim), int(y_dim), int(n_mesh))
+        dev = data.states.device
+        T = B * len(ids) * n_mesh * n_mesh
+        probes = min(T, int(max_probes) if max_probes is not None else self.FIELD_MAX_PROBES)
+        edge_cap = int(max_edges) if max_edges is not None else max(self.FIELD_MAX_EDGES, N - 1)
+        if edge_cap < N - 1:
+            raise ValueError(f'max_edges must be >= nodes_per_graph - 1 = {N - 1} (the edges one probe can have), got {edge_cap}')
+
+        ops.sync_gemm_impl()
+        spec = self.cbf.feat_transformer.module_0.net_spec(self.cbf.feat_2_CBF)
+        layers = spec.all_layers()
+        d = native.FieldDesc()
+        ctypes.memmove(ctypes.byref(d.cbf), ctypes.byref(native.make_net_desc(spec, 0, None)), ctypes.sizeof(native.NetDesc))
+        d.cbf.refresh_weights = 1 if native._weights_stale(layers) else 0
+        ctypes.memmove(ctypes.byref(d.env), ctypes.byref(env._cfg(B)), ctypes.sizeof(_C.EnvCfg))
+        st, ld = ops._mat(data.states.detach())
+        x = data.x.detach().contiguous()
+        if relink:                                       # the given edges are not read
+            ei, rowptr, E = None, None, 0
+        else:
+            ei = data.edge_index.contiguous()
+            E = int(ei.shape[1])
+            rowptr = cached_rowptr(data.edge_index, int(x.shape[0]))
+        agents_t = torch.tensor(ids, device=dev, dtype=torch.int32)
+        xs_t = torch.from_numpy(np.asarray(xs, dtype=np.float32)).to(dev)
+        ys_t = torch.from_numpy(np.asarray(ys, dtype=np.float32)).to(dev)
+        d.states, d.x, d.num_edges = st.data_ptr(), x.data_ptr(), E
+        d.edge_index, d.rowptr = (ei.data_ptr() if E else None), (rowptr.data_ptr() if rowptr is not None else None)
+        d.agents, d.xs, d.ys = agents_t.data_ptr(), xs_t.data_ptr(), ys_t.data_ptr()
+        d.max_edges, d.max_probes = edge_cap, probes
+        d.ld_state, d.state_dim, d.pos_dim, d.graph_metric = ld, sd, env.POS_DIM, env.GRAPH_METRIC
+        d.comm_radius, d.relink = float(env._params['comm_radius']), 1 if relink else 0
+        d.num_probe_agents, d.x_dim, d.y_dim, d.nx, d.ny = len(ids), int(x_dim), int(y_dim), int(n_mesh), int(n_mesh)
+        return d, (st, x, ei, rowptr, agents_t, xs_t, ys_t, layers), xs, ys, B, len(ids), T
+
     # ---- checkpoints (file names and keys of gcbf.py:249-258) ------------------------------------------
     def save(self, save_dir: str):
         os.makedirs(save_dir, exist_ok=True)

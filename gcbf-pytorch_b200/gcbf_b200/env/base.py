@@ -26,6 +26,16 @@ def lqr(A: np.ndarray, B: np.ndarray, Q: np.ndarray, R: np.ndarray) -> np.ndarra
     return inv(B.T @ X @ B + R) @ (B.T @ X @ A)
 
 
+def plot_box(points: np.ndarray, agent_radius: float) -> Tuple[np.ndarray, np.ndarray]:
+    """The square x-y plotting box the reference's SimpleCar / DubinsCar `reset()` stores for `state_lim` (simple_car.py:136-142,
+    dubins_car.py:491-497): the bounding box of `points` (agent positions, goals[, obstacle positions], float32 [k, 2]) grown by
+    5 agent radii, then widened along its shorter side to a square about the same centre.  Returns (xy_min, xy_max)."""
+    xy_min = np.min(points, axis=0) - agent_radius * 5
+    xy_max = np.max(points, axis=0) + agent_radius * 5
+    max_interval = (xy_max - xy_min).max()
+    return xy_min - 0.5 * (max_interval - (xy_max - xy_min)), xy_max + 0.5 * (max_interval - (xy_max - xy_min))
+
+
 class _StepFunction(torch.autograd.Function):
     """x+ = x + dt f(x, clamp(u + u_ref(x))): forward_graph's state update with its VJP to the action."""
 
@@ -60,6 +70,7 @@ class MultiAgentEnv(ABC):
     RADIUS_KEY = 'car_radius'
     GRAPH_METRIC = 1          # 0: squared distance (torch_cluster), 1: torch.norm then compare
     GOAL_DIM = 2              # goal columns the kernels read (SimpleCar 2, DubinsCar 2, SimpleDrone 6)
+    _xy_min = _xy_max = None  # x-y plotting box of state_lim (SimpleCar / DubinsCar: set by reset(), see plot_box)
 
     def __init__(self, num_agents: int, device: torch.device, dt: float = 0.03, params: Optional[dict] = None,
                  max_neighbors: Optional[int] = None):
@@ -143,6 +154,11 @@ class MultiAgentEnv(ABC):
 
     def _gain(self) -> Optional[Tensor]:
         return None
+
+    def _plot_box(self):
+        if self._xy_min is None:
+            raise RuntimeError(f'{self.ENV_NAME}.state_lim: its x-y box is set by reset(); call reset() first or pass the limits explicitly')
+        return self._xy_min, self._xy_max
 
     def set_goal(self, goal: Tensor):
         """Install the goal set [num_agents, goal_dim] (the reference keeps it in `env._goal`).  Rows narrower than the

@@ -9,7 +9,7 @@ from torch import Tensor
 
 from ..data import Data
 from ._sampling import sample_separated
-from .base import MultiAgentEnv
+from .base import MultiAgentEnv, plot_box
 
 
 class DubinsCar(MultiAgentEnv):
@@ -41,6 +41,14 @@ class DubinsCar(MultiAgentEnv):
         hi = torch.ones(2, device=self.device) * 2.
         return -hi, hi
 
+    @property
+    def state_lim(self) -> Tuple[Tensor, Tensor]:
+        """(low, high) of [x, y, theta, v] for plotting (reference dubins_car.py:748-756): the x-y box of the last reset()."""
+        xy_min, xy_max = self._plot_box()
+        low_lim = torch.tensor([xy_min[0], xy_min[1], -10, -10], device=self.device)
+        high_lim = torch.tensor([xy_max[0], xy_max[1], 10, 10], device=self.device)
+        return low_lim, high_lim
+
     def make_graph(self, states: Tensor) -> Data:
         n, o = self.num_agents, self._num_obs
         B = states.shape[0] // (n + o)
@@ -65,6 +73,7 @@ class DubinsCar(MultiAgentEnv):
         goal_heading = torch.rand(self.num_agents, 1) * 2 * math.pi - math.pi
         self.set_goal(torch.cat([goal_xy, goal_heading, torch.zeros(self.num_agents, 1)], dim=1))
         states = torch.cat([agents, obs], dim=0).to(self.device)
+        self._xy_min, self._xy_max = plot_box(torch.cat([pos, goal_xy, obs[:, :2]], dim=0).float().numpy(), R)
         self._data = self.add_communication_links(self.make_graph(states))
         return self._data
 

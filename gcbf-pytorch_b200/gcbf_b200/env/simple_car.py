@@ -8,7 +8,7 @@ from torch import Tensor
 
 from ..data import Data
 from ._sampling import sample_separated
-from .base import MultiAgentEnv, lqr
+from .base import MultiAgentEnv, lqr, plot_box
 
 
 class SimpleCar(MultiAgentEnv):
@@ -40,6 +40,16 @@ class SimpleCar(MultiAgentEnv):
             self._K = torch.from_numpy(lqr(A, B, np.eye(4), np.eye(2))).to(self.device, torch.float32).contiguous()
         return self._K
 
+    @property
+    def state_lim(self) -> Tuple[Tensor, Tensor]:
+        """(low, high) of [x, y, vx, vy] for plotting (reference simple_car.py:254-262): the x-y box of the last reset()."""
+        xy_min, xy_max = self._plot_box()
+        low_lim = torch.tensor([xy_min[0], xy_min[1], -self._params['speed_limit'], -self._params['speed_limit']],
+                               device=self.device)
+        high_lim = torch.tensor([xy_max[0], xy_max[1], self._params['speed_limit'], self._params['speed_limit']],
+                                device=self.device)
+        return low_lim, high_lim
+
     def make_graph(self, states: Tensor) -> Data:
         return Data(x=torch.zeros_like(states), pos=states[:, :2], states=states)
 
@@ -47,7 +57,9 @@ class SimpleCar(MultiAgentEnv):
         self._t = 0
         side, R = self._params['area_size'], self._params['car_radius']
         pos = sample_separated(self.num_agents, 2, side, 4 * R)
-        self.set_goal(sample_separated(self.num_agents, 2, side, 4 * R))
+        goal = sample_separated(self.num_agents, 2, side, 4 * R)
+        self.set_goal(goal)
+        self._xy_min, self._xy_max = plot_box(torch.cat([pos, goal], dim=0).float().numpy(), R)
         states = torch.cat([pos, torch.zeros(self.num_agents, 2)], dim=1).to(self.device)
         self._data = self.add_communication_links(self.make_graph(states))
         return self._data

@@ -49,6 +49,14 @@ class SimpleDrone(MultiAgentEnv):
             self._K = torch.from_numpy(K).to(self.device, torch.float32).contiguous()
         return self._K
 
+    @property
+    def state_lim(self) -> Tuple[Tensor, Tensor]:
+        """(low, high) of [x, y, z, vx, vy, vz] for plotting (reference simple_drone.py:44-45, 335-341): the cube [0, area_size]^3."""
+        xyz_min, xyz_max = np.array([0, 0, 0]), np.ones(3) * self._params['area_size']
+        low_lim = torch.tensor([xyz_min[0], xyz_min[1], xyz_min[2], -10, -10, -10], device=self.device)
+        high_lim = torch.tensor([xyz_max[0], xyz_max[1], xyz_max[2], 10, 10, 10], device=self.device)
+        return low_lim, high_lim
+
     def make_graph(self, states: Tensor) -> Data:
         n = self.num_agents
         B = states.shape[0] // (2 * n)

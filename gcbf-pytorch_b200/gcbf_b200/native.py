@@ -72,6 +72,15 @@ class H16Desc(ctypes.Structure):
                 ('amax_col_stride', c_int32), ('pad_', c_int32)]
 
 
+class FieldDesc(ctypes.Structure):
+    """mirror of `gcbf_field_desc`"""
+    _fields_ = [('cbf', NetDesc), ('env', _C.EnvCfg), ('states', P), ('x', P), ('edge_index', P), ('rowptr', P), ('num_edges', c_int64),
+                ('agents', P), ('xs', P), ('ys', P), ('max_edges', c_int64), ('ld_state', c_int32), ('state_dim', c_int32),
+                ('pos_dim', c_int32), ('graph_metric', c_int32), ('comm_radius', c_float), ('relink', c_int32),
+                ('num_probe_agents', c_int32), ('x_dim', c_int32), ('y_dim', c_int32), ('nx', c_int32), ('ny', c_int32),
+                ('max_probes', c_int32)]
+
+
 class TimeRec(ctypes.Structure):
     """mirror of `gcbf_time_rec`"""
     _fields_ = [('ms', c_double), ('flops', c_double), ('kind', c_int32), ('M', c_int32), ('N', c_int32), ('K', c_int32)]
@@ -97,6 +106,10 @@ SIGS = {
     'gcbf_apply_batch_workspace_bytes': (c_size_t, [POINTER(StepDesc), POINTER(StepBatch)]),
     'gcbf_apply_batch': (c_int, [POINTER(StepDesc), POINTER(StepBatch), c_float, c_float, P, c_int, P, c_int, P, POINTER(c_int), P, c_size_t,
                                  P]),
+    'gcbf_cbf_field_workspace_bytes': (c_size_t, [POINTER(FieldDesc)]),
+    'gcbf_cbf_field': (c_int, [POINTER(FieldDesc), P, POINTER(c_int64), P, c_size_t, P]),
+    'gcbf_cbf_field_probe_count': (c_int, [POINTER(FieldDesc), P, P]),
+    'gcbf_cbf_field_probe_fill': (c_int, [POINTER(FieldDesc), P, P, c_int64, P, P]),
     'gcbf_linear_fwd_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P]),
     'gcbf_linear_bwd_data_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
                                        c_int, c_int, c_int, P]),

@@ -50,7 +50,7 @@ const char* gcbf_last_error(void);
 int gcbf_abi_version(void);
 /* sizeof() of ABI structure number `which` as the library was compiled (0 gcbf_env_cfg, 1 gcbf_linear_desc, 2 gcbf_net_desc,
  * 3 gcbf_step_desc, 4 gcbf_step_batch, 5 gcbf_step_out, 6 gcbf_net_ctx, 7 gcbf_mlp_ctx, 8 gcbf_step_ctx, 9 gcbf_time_rec,
- * 10 gcbf_sn_layer, 11 gcbf_split_desc, 12 gcbf_h16; 0 for unknown): bindings check their mirrors against it */
+ * 10 gcbf_sn_layer, 11 gcbf_split_desc, 12 gcbf_h16, 13 gcbf_field_desc; 0 for unknown): bindings check their mirrors against it */
 size_t gcbf_abi_struct_size(int which);
 /* 1 if the library was built with the wgmma (3xFP16) GEMM path compiled in, else 0 (ABI v5: was gcbf_has_tcgen05) */
 int gcbf_has_wgmma(void);
@@ -450,6 +450,51 @@ int gcbf_apply(const gcbf_step_desc* d, const gcbf_step_batch* graph, float lr, 
 size_t gcbf_apply_batch_workspace_bytes(const gcbf_step_desc* d, const gcbf_step_batch* batch);
 int gcbf_apply_batch(const gcbf_step_desc* d, const gcbf_step_batch* batch, float lr, float rand, const float* noise, int max_iter,
                      float* action, int ld_action, int32_t* rounds, int* iterations, void* workspace, size_t workspace_bytes, void* stream);
+
+/* CBF level-set field: h of chosen agents over a grid of two state dimensions -- the data of plot_cbf_contour
+ * (gcbf/trainer/utils.py:226-298, what plot_cbf.py draws), for B graphs and A agents in one call.
+ * A probe t = ((b * num_probe_agents + ai) * ny + iy) * nx + ix is graph b's agent a = agents[ai] with state[x_dim] = xs[ix] and
+ * state[y_dim] = ys[iy] (utils.py:262-267; xs, ys fp32, the rounding of the reference's write into its fp32 state tensor), everyone else
+ * fixed; h[t] = CBFGNN(graph)[a] evaluated on that state (utils.py:268-273).  h_a depends only on a's in-edges and x_a, so instead of
+ * n_mesh^2 copies of every graph each probe becomes one extra target node with its own in-edges (a "probe graph"):
+ *   relink == 0  the in-edges of a in the given edge_index, in their order, with edge_attr = g(s_j) - g(s'_t) recomputed
+ *                (the reference's fixed edge_index, utils.py:268-269; default);
+ *   relink != 0  every node j != a of graph b inside the radius of s'_t under the K1 rule (metric / comm_radius as the radius graph:
+ *                SimpleCar agents only, DubinsCar / SimpleDrone agents and obstacles), ascending j: the edges gcbf_radius_graph_*
+ *                would give target a on the moved state.
+ * The probes go through the CBF net (gcbf_net_forward's chain, GEMM dispatch unchanged) in chunks of at most max_probes probes and
+ * max_edges probe edges (the workspace is sized for min(max_edges, chunk probes * (nodes_per_graph - 1)) edges); every chunk uses the 1/sigma of ONE spectral-norm power iteration done at the start of the call, so a call
+ * advances the CBF's u, v exactly once, as the reference's single cbf(plot_data) does.  ONE host sync per call: the per-probe edge
+ * counts are counted on the device for all probes and read back to split the probes into chunks (stream-ordered: the call returns
+ * with the field still being computed).  max_edges must be < 2^31 and at least the largest probe's edge count (nodes_per_graph - 1
+ * always suffices), else GCBF_E_INVALID.  Preconditions not checked on the device: agent ids in [0, num_agents), the given graph's
+ * edge_index target-sorted with rowptr its CSR over all num_graphs * nodes_per_graph nodes (fixed mode).
+ * gcbf_cbf_field_workspace_bytes: dry run of the call for these sizes (0 for an invalid descriptor); gcbf_cbf_field checks the size
+ * before launching anything. */
+typedef struct gcbf_field_desc {
+  gcbf_net_desc cbf;                      /* the CBF net (n_head > 0, one output column) */
+  gcbf_env_cfg env;                       /* env, num_graphs, nodes_per_graph, num_agents (the radii / dt are not used) */
+  const float* states; const float* x;    /* [num_graphs * nodes_per_graph, ld_state], [.., node_dim] */
+  const int64_t* edge_index; const int32_t* rowptr; int64_t num_edges;   /* the given graph (read in fixed mode only) */
+  const int32_t* agents;                  /* [num_probe_agents] device int32, ids in [0, num_agents) */
+  const float* xs; const float* ys;       /* [nx], [ny] device fp32 grid values */
+  int64_t max_edges;                      /* probe-edge bound of a chunk */
+  int32_t ld_state, state_dim, pos_dim, graph_metric;
+  float comm_radius; int32_t relink;
+  int32_t num_probe_agents, x_dim, y_dim, nx, ny;
+  int32_t max_probes;                     /* probe bound of a chunk */
+} gcbf_field_desc;
+size_t gcbf_cbf_field_workspace_bytes(const gcbf_field_desc* d);
+/* h [num_graphs * num_probe_agents * ny * nx] fp32; info (host int64[2], optional) = chunks the probes ran in, probe edges in all */
+int gcbf_cbf_field(const gcbf_field_desc* d, float* h, int64_t* info, void* workspace, size_t workspace_bytes, void* stream);
+/* The probe graphs themselves, for inspection (same two-call protocol and edge order as gcbf_radius_graph_count / _fill; d->cbf and the
+ * chunk bounds are not read): count writes rowptr[T + 1] (int32 exclusive scan of the per-probe edge counts, T = num_graphs *
+ * num_probe_agents * ny * nx; rowptr[T] is the total, which must stay below 2^31); fill writes edge_index [2, num_edges] with source =
+ * the original node id (b * nodes_per_graph + j) and target = the probe id t, sorted (t asc, source asc), and edge_attr [num_edges,
+ * edge_dim] = g(s_source) - g(s'_t).  These are the edges and features gcbf_cbf_field feeds the CBF. */
+int gcbf_cbf_field_probe_count(const gcbf_field_desc* d, int32_t* rowptr, void* stream);
+int gcbf_cbf_field_probe_fill(const gcbf_field_desc* d, const int32_t* rowptr, int64_t* edge_index, int64_t num_edges, float* edge_attr,
+                              void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * MACBF, the paper's baseline algorithm (gcbf/algo/macbf.py:20-239; SURVEY 8f-4): the kernels it needs beyond the ones above.
