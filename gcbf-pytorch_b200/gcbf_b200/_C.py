@@ -32,6 +32,15 @@ class SplitDesc(ctypes.Structure):
                 ('amax_slot', c_void_p), ('dst', c_void_p)]
 
 
+class ResetDesc(ctypes.Structure):
+    """mirror of `gcbf_reset_desc`"""
+    _fields_ = [('seed', c_ulonglong), ('states', c_void_p), ('goals', c_void_p), ('step_count', c_void_p), ('episode', c_void_p),
+                ('failed', c_void_p), ('reach', c_void_p), ('env', c_int32), ('num_envs', c_int32), ('num_agents', c_int32),
+                ('num_obs', c_int32), ('ld_state', c_int32), ('ld_goal', c_int32), ('goal_dim', c_int32), ('max_steps', c_int32),
+                ('max_tries', c_int32), ('first_env', c_int32), ('area', c_float), ('agent_dist2', c_float), ('goal_dist2', c_float),
+                ('clear2', c_float), ('obs_speed_limit', c_float), ('pad_', c_float)]
+
+
 P = c_void_p  # every device pointer travels as void*
 _SIGS = {
     'gcbf_last_error': (c_char_p, []),
@@ -98,6 +107,8 @@ _SIGS = {
     'gcbf_loss_grads_hdot': (c_int, [P, P, P, c_int, P, P, c_int64, c_float, c_float, c_float, c_float, c_float, c_float, P, P, P, P, P, P]),
     'gcbf_macbf_loss_grads': (c_int, [P, P, P, P, c_int64, P, c_int, c_int64, c_float, c_float, c_float, c_float, c_float, c_float,
                                       c_float, P, P, P, P, P, P]),
+    # batched episode reset (csrc/reset.cu)
+    'gcbf_env_reset_batch': (c_int, [POINTER(ResetDesc), P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

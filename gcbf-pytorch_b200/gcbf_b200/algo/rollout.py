@@ -10,8 +10,13 @@ single graph -> reach-freeze branch), and an append of all `num_envs` graphs to 
 safe / unsafe flags staying on the device.  The only host sync per step is the batched radius graph's edge count.
 
 Episode semantics follow the reference's `step`: an env is done when t reaches max_episode_steps or when all its agents are
-within dist2goal of their goals (checked on the device; the flags are read back every `reset_check_every` steps, so a finished
-env may run a few extra steps before it is re-sampled -- its agents are frozen at their goals by then).
+within dist2goal of their goals.  Two ways to start the next episode:
+  - host resets (reset_seed=None, the default): env.reset() per finished env; "all agents reached" is checked on the device and the
+    flags are read back every `reset_check_every` steps, so a finished env may run a few extra steps before it is re-sampled (its
+    agents are frozen at their goals by then);
+  - device resets (reset_seed=<int>): per-env step and episode counters live on the device, and after every dynamics step ONE
+    `gcbf_env_reset_batch` launch (env/device_reset.py) re-samples every done env in place, so it starts its next episode on the very
+    next step.  No host reads of the done flags.
 """
 import ctypes
 from typing import Callable, Dict, Optional, Sequence
@@ -25,9 +30,16 @@ from ..data import Data
 
 class VectorRollout:
     def __init__(self, env, algo, num_envs: int, reset_check_every: int = 16, states: Optional[torch.Tensor] = None,
-                 goals: Optional[torch.Tensor] = None):
+                 goals: Optional[torch.Tensor] = None, reset_seed: Optional[int] = None):
         """states [num_envs * N, s] / goals [num_envs * n, goal_dim]: explicit initial conditions (e.g. synthetic BASELINE states:
-        the reference's rejection sampler cannot place >~ 290 agents, SURVEY section 0); default: env.reset() per env."""
+        the reference's rejection sampler cannot place >~ 290 agents, SURVEY section 0); default: env.reset() per env.
+
+        reset_seed: None keeps the host resets above.  An integer switches to device resets: the initial states are episode 0 of every
+        env drawn by `gcbf_env_reset_batch` with this seed, and every done env is re-sampled on the device right after the step that
+        finished it (env e's episode k depends only on (reset_seed, e, k)).  In that mode the per-env step counters `t_dev` and
+        episode counters `episode` are device tensors and the host array `self.t` is NOT authoritative (it counts steps since
+        construction); a reset that cannot place its points raises RuntimeError at the next step's edge-count sync (or
+        `check_resets()`)."""
         self.env, self.algo, self.B = env, algo, int(num_envs)
         self.n, self.N = env.num_agents, env.nodes_per_graph
         self.dev = env.device
@@ -38,11 +50,49 @@ class VectorRollout:
         self.steps = 0
         self._done_host = None
         self._auto_reset = states is None
-        if states is None:
+        self.reset_seed = None if reset_seed is None else int(reset_seed)
+        if self.reset_seed is not None:
+            if states is not None:
+                raise ValueError('VectorRollout: reset_seed draws the initial states on the device; do not pass states / goals')
+            self._auto_reset = False
+            self._init_device_resets()
+        elif states is None:
             self.reset()
         else:
             self.states = states.to(self.dev, torch.float32).contiguous().clone()
             self.goals = goals.to(self.dev, torch.float32).contiguous().clone()
+
+    # ---- device side: episode management by gcbf_env_reset_batch ------------------------------------------------------------
+    def _init_device_resets(self):
+        from ..env.device_reset import reset_spec
+        env, B = self.env, self.B
+        self.states = torch.zeros(B * self.N, env.state_dim, device=self.dev, dtype=torch.float32)
+        self.goals = torch.zeros(B * self.n, reset_spec(env)['goal_dim'], device=self.dev, dtype=torch.float32)
+        self.t_dev = torch.full((B,), int(env.max_episode_steps), device=self.dev, dtype=torch.int32)    # every env is due
+        self.episode = torch.full((B,), -1, device=self.dev, dtype=torch.int32)                          # -> episode 0
+        self._failed = torch.zeros(B, device=self.dev, dtype=torch.int32)
+        self._failed_host = torch.zeros(B, dtype=torch.int32).pin_memory()
+        self._failed_ev = None
+        self._device_reset(None)
+        # as after host resets, the env's own goal set (read where a batch carries no per-graph goals) is the last env's
+        env.set_goal(self.goals[(B - 1) * self.n:].clone())
+
+    def _device_reset(self, reach: Optional[torch.Tensor]):
+        """One gcbf_env_reset_batch launch over the batch and an asynchronous copy of the failure flags (read by check_resets)."""
+        from ..env.device_reset import reset_batch
+        reset_batch(self.env, self.states, self.goals, self.t_dev, self.episode, self._failed, self.reset_seed, reach=reach)
+        self._failed_host.copy_(self._failed, non_blocking=True)
+        self._failed_ev = torch.cuda.Event()
+        self._failed_ev.record()
+
+    def check_resets(self):
+        """Raise RuntimeError if the last device reset could not place an env's agents or goals (waits for that reset only)."""
+        if self.reset_seed is None or self._failed_ev is None:
+            return
+        from ..env.device_reset import raise_on_failure
+        self._failed_ev.synchronize()
+        self._failed_ev = None
+        raise_on_failure(self.env, self._failed_host.numpy())
 
     # ---- host side: initial conditions (the reference's rejection sampler, one env at a time) -------------------------
     def _sample_one(self):
@@ -65,6 +115,8 @@ class VectorRollout:
     def keep(self, which):
         """Keep only the environments `which` (ascending indices into the current batch), in that order: the others drop out of the
         batch and cost nothing from the next step on."""
+        if self.reset_seed is not None:
+            raise NotImplementedError('VectorRollout.keep: device resets draw by env id; dropping envs is not supported with reset_seed')
         idx = torch.as_tensor(np.asarray(which, dtype=np.int64))
         nodes = (idx.unsqueeze(1) * self.N + torch.arange(self.N)).reshape(-1).to(self.dev)
         agents = (idx.unsqueeze(1) * self.n + torch.arange(self.n)).reshape(-1).to(self.dev)
@@ -78,7 +130,9 @@ class VectorRollout:
         """All envs advance one step under the actor (each env's action zeroed with probability `prob`, the reference's
         exploration schedule gcbf.py:131-132), or under `policy(batch)` -- e.g. `algo.apply_batch`, the test-time controller --
         which gets the collated batch with u_ref and the per-env goal sets (`batch.goal`).  Returns device tensors: reach [B, n],
-        collision [B, n] (after the step), is_safe [B] (before the step: what the stored graph is labelled with, gcbf.py:133-137)."""
+        collision [B, n] (after the step), is_safe [B] (before the step: what the stored graph is labelled with, gcbf.py:133-137),
+        action, and the step's inputs states [B * N, s] (pre-step), u_ref [B * n, a] and goals [B * n, goal_dim] (with device resets,
+        tensors no later step or reset writes to); plus edge_count."""
         if policy is None:
             with torch.no_grad():
                 return self._step(prob, store, None)
@@ -93,6 +147,8 @@ class VectorRollout:
         u_ref = torch.empty(B * n, a_dim, device=self.dev, dtype=torch.float32)
         _C.call('gcbf_u_ref_multi', ctypes.byref(cfg), _C.ptr(st), ld, _C.ptr(goal), ldg, _C.ptr(env._gain()), _C.ptr(u_ref))
         data = env.add_communication_links(env.make_graph(self.states))          # ONE radius graph + edge features for all envs
+        if self.reset_seed is not None:
+            self.check_resets()                      # the edge count above synchronised: the last reset's flags are on the host
         data.update(Data(u_ref=u_ref))
         if policy is None:
             action = self.algo.actor(data)                                       # ONE actor forward (block-diagonal batch)
@@ -122,9 +178,17 @@ class VectorRollout:
         collision = env._masks(coll_data)[2].view(B, n)
         self.t += 1
         self.steps += 1
+        out = dict(reach=reach, collision=collision, is_safe=is_safe, action=action, states=st, u_ref=u_ref, goals=self.goals,
+                   edge_count=int(data.edge_index.shape[1]))
+        if self.reset_seed is not None:
+            # done envs start their next episode right away: counters and re-sampling on the device, no host read of the flags
+            self.goals = self.goals.clone()          # the returned goals stay those of this step
+            self.t_dev += 1
+            self._device_reset(reach)
+            return out
         # episode ends: time limit known on the host; "all agents reached" read back with a delay (no sync in the common step)
         if not self._auto_reset:
-            return dict(reach=reach, collision=collision, is_safe=is_safe, action=action, edge_count=int(data.edge_index.shape[1]))
+            return out
         if self._done_host is not None and self.steps % self.reset_check_every == 0:
             flags, ev = self._done_host
             ev.synchronize()
@@ -141,7 +205,7 @@ class VectorRollout:
         timeout = np.nonzero(self.t >= env.max_episode_steps)[0].tolist()
         if timeout:
             self.reset(timeout)
-        return dict(reach=reach, collision=collision, is_safe=is_safe, action=action, edge_count=int(data.edge_index.shape[1]))
+        return out
 
 
 def evaluate_episodes(env, algo, seeds: Sequence[int], rand: Optional[float] = 30, max_iter: int = 30,

@@ -70,6 +70,13 @@ class MultiAgentEnv(ABC):
     RADIUS_KEY = 'car_radius'
     GRAPH_METRIC = 1          # 0: squared distance (torch_cluster), 1: torch.norm then compare
     GOAL_DIM = 2              # goal columns the kernels read (SimpleCar 2, DubinsCar 2, SimpleDrone 6)
+    # reset(): agents / goals pairwise farther than RESET_*_SPACING agent radii, and (envs with obstacles) farther than
+    # RESET_CLEARANCE[0] * R + RESET_CLEARANCE[1] * obs_point_r from every obstacle; goal rows of RESET_GOAL_DIM columns.  The device
+    # reset (env/device_reset.py) reads the same attributes.
+    RESET_AGENT_SPACING = 4
+    RESET_GOAL_SPACING = 4
+    RESET_CLEARANCE = (2, 2)
+    RESET_GOAL_DIM = 2
     _xy_min = _xy_max = None  # x-y plotting box of state_lim (SimpleCar / DubinsCar: set by reset(), see plot_box)
 
     def __init__(self, num_agents: int, device: torch.device, dt: float = 0.03, params: Optional[dict] = None,

@@ -17,6 +17,8 @@ class DubinsCar(MultiAgentEnv):
     POS_DIM = 2
     RADIUS_KEY = 'car_radius'
     GRAPH_METRIC = 1
+    RESET_GOAL_SPACING = 5
+    RESET_GOAL_DIM = 4        # goals carry a heading: [x, y, theta, 0]
 
     state_dim = property(lambda self: 4)
     edge_dim = property(lambda self: 5)
@@ -60,14 +62,14 @@ class DubinsCar(MultiAgentEnv):
         self._t = 0
         p = self._params
         side, R = p['area_size'], p['car_radius']
-        clear = 2 * R + 2 * p['obs_point_r']
+        clear = self.RESET_CLEARANCE[0] * R + self.RESET_CLEARANCE[1] * p['obs_point_r']
         obs = torch.rand(self._num_obs, 4)
         obs[:, :2] *= side
         obs[:, 2] *= 2 * math.pi
         obs[:, 3] *= p['obs_speed_limit']
         self._obs = obs.to(self.device)
-        pos = sample_separated(self.num_agents, 2, side, 4 * R, obs[:, :2], clear)
-        goal_xy = sample_separated(self.num_agents, 2, side, 5 * R, obs[:, :2], clear)
+        pos = sample_separated(self.num_agents, 2, side, self.RESET_AGENT_SPACING * R, obs[:, :2], clear)
+        goal_xy = sample_separated(self.num_agents, 2, side, self.RESET_GOAL_SPACING * R, obs[:, :2], clear)
         heading = torch.rand(self.num_agents, 1) * 2 * math.pi - math.pi
         agents = torch.cat([pos, heading, torch.zeros(self.num_agents, 1)], dim=1)
         goal_heading = torch.rand(self.num_agents, 1) * 2 * math.pi - math.pi

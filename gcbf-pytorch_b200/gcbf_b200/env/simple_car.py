@@ -56,8 +56,8 @@ class SimpleCar(MultiAgentEnv):
     def reset(self) -> Data:
         self._t = 0
         side, R = self._params['area_size'], self._params['car_radius']
-        pos = sample_separated(self.num_agents, 2, side, 4 * R)
-        goal = sample_separated(self.num_agents, 2, side, 4 * R)
+        pos = sample_separated(self.num_agents, 2, side, self.RESET_AGENT_SPACING * R)
+        goal = sample_separated(self.num_agents, 2, side, self.RESET_GOAL_SPACING * R)
         self.set_goal(goal)
         self._xy_min, self._xy_max = plot_box(torch.cat([pos, goal], dim=0).float().numpy(), R)
         states = torch.cat([pos, torch.zeros(self.num_agents, 2)], dim=1).to(self.device)

@@ -15,6 +15,7 @@ class SimpleDrone(MultiAgentEnv):
     ENV_NAME = 'SimpleDrone'
     POS_DIM = 3
     GOAL_DIM = 6
+    RESET_GOAL_DIM = 6
     RADIUS_KEY = 'drone_radius'
     GRAPH_METRIC = 1
 
@@ -68,11 +69,11 @@ class SimpleDrone(MultiAgentEnv):
         self._t = 0
         p = self._params
         side, R = p['area_size'], p['drone_radius']
-        clear = 2 * R + 2 * p['obs_point_r']
+        clear = self.RESET_CLEARANCE[0] * R + self.RESET_CLEARANCE[1] * p['obs_point_r']
         n = self.num_agents
         obs_pos = torch.rand(n, 3) * side
-        pos = sample_separated(n, 3, side, 4 * R, obs_pos, clear)
-        goal = sample_separated(n, 3, side, 4 * R, obs_pos, clear)
+        pos = sample_separated(n, 3, side, self.RESET_AGENT_SPACING * R, obs_pos, clear)
+        goal = sample_separated(n, 3, side, self.RESET_GOAL_SPACING * R, obs_pos, clear)
         self.set_goal(torch.cat([goal, torch.zeros(n, 3)], dim=1))
         agents = torch.cat([pos, torch.zeros(n, 3)], dim=1)
         obstacles = torch.cat([obs_pos, torch.zeros(n, 3)], dim=1)

@@ -50,7 +50,8 @@ const char* gcbf_last_error(void);
 int gcbf_abi_version(void);
 /* sizeof() of ABI structure number `which` as the library was compiled (0 gcbf_env_cfg, 1 gcbf_linear_desc, 2 gcbf_net_desc,
  * 3 gcbf_step_desc, 4 gcbf_step_batch, 5 gcbf_step_out, 6 gcbf_net_ctx, 7 gcbf_mlp_ctx, 8 gcbf_step_ctx, 9 gcbf_time_rec,
- * 10 gcbf_sn_layer, 11 gcbf_split_desc, 12 gcbf_h16, 13 gcbf_field_desc; 0 for unknown): bindings check their mirrors against it */
+ * 10 gcbf_sn_layer, 11 gcbf_split_desc, 12 gcbf_h16, 13 gcbf_field_desc, 14 gcbf_reset_desc; 0 for unknown): bindings check their
+ * mirrors against it */
 size_t gcbf_abi_struct_size(int which);
 /* 1 if the library was built with the wgmma (3xFP16) GEMM path compiled in, else 0 (ABI v5: was gcbf_has_tcgen05) */
 int gcbf_has_wgmma(void);
@@ -495,6 +496,34 @@ int gcbf_cbf_field(const gcbf_field_desc* d, float* h, int64_t* info, void* work
 int gcbf_cbf_field_probe_count(const gcbf_field_desc* d, int32_t* rowptr, void* stream);
 int gcbf_cbf_field_probe_fill(const gcbf_field_desc* d, const int32_t* rowptr, int64_t* edge_index, int64_t num_edges, float* edge_attr,
                               void* stream);
+
+/* Batched episode reset of a vectorised rollout (num_envs copies of one env, nodes_per_graph = num_agents + num_obs rows each, agents
+ * first): in ONE launch, every env e that is done -- step_count[e] >= max_steps, or (reach != NULL) all reach[e * num_agents + i] set,
+ * the reference's `done` of env.step -- is re-sampled in place with the algorithm of that env's reset() (gcbf/env/<env>.py):
+ *   SimpleCar    agents, then goals in [0, area]^2, each set with pairwise spacing > agent_dist / goal_dist;
+ *   DubinsCar    num_obs obstacles [x, y, theta, v] uniform in [0, area]^2 x [0, 2 pi) x [0, obs_speed_limit); agents and goals as above
+ *                and farther than the clearance from every obstacle; agent / goal headings uniform in [-pi, pi), speeds 0;
+ *   SimpleDrone  num_obs static obstacles uniform in [0, area]^3; agents and goals as DubinsCar; velocities 0, goal columns past 3 zero.
+ * Rejection rule: candidate c is rejected iff sum_d (p_d - c_d)^2 <= min_dist2 for a placed point p (clear2 for an obstacle), every
+ * operation rounded on its own, d ascending.  The candidates of a point set are tried in order; a set whose first max_tries candidates
+ * do not place all its points sets failed[e] (1 agents, 2 goals; 0 on success).  Random numbers: Philox4x32-10, key = seed, counter =
+ * (draw index, first_env + e, new episode number, stream: 0 obstacles, 1 agents, 2 goals, 3 headings), uniform = (word >> 8) 2^-24;
+ * a reset depends only on (seed, first_env + e, episode, stream, draw index).  A reset env gets step_count[e] = 0 and episode[e] + 1;
+ * an env that is not done is left untouched.  No host sync; one warp and (num_agents + num_obs) * pos_dim floats of shared memory per env. */
+typedef struct gcbf_reset_desc {
+  uint64_t seed;
+  float* states;              /* [num_envs * (num_agents + num_obs), ld_state] */
+  float* goals;               /* [num_envs * num_agents, ld_goal]; columns [0, goal_dim) are written */
+  int32_t* step_count;        /* [num_envs] device */
+  int32_t* episode;           /* [num_envs] device: the current episode; a reset draws episode[e] + 1 */
+  int32_t* failed;            /* [num_envs] device, written for every reset env */
+  const uint8_t* reach;       /* [num_envs * num_agents] device, or NULL: done on the step counter alone */
+  int32_t env, num_envs, num_agents, num_obs;
+  int32_t ld_state, ld_goal, goal_dim, max_steps;
+  int32_t max_tries, first_env;
+  float area, agent_dist2, goal_dist2, clear2, obs_speed_limit, pad_;
+} gcbf_reset_desc;
+int gcbf_env_reset_batch(const gcbf_reset_desc* d, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * MACBF, the paper's baseline algorithm (gcbf/algo/macbf.py:20-239; SURVEY 8f-4): the kernels it needs beyond the ones above.
