@@ -18,13 +18,17 @@
 //
 // Kernel.  One CTA per 128 x BN output tile (BN = 128 or 256) and contraction split, three warpgroups: warp 0 of warpgroup 0
 // is the TMA producer (cp.async.bulk.tensor 2-D boxes into swizzled shared memory, STAGES-deep mbarrier ring), warpgroups
-// 1 and 2 each own 64 rows of the tile and issue m64n128k16 wgmma.  A 256-wide tile is computed as two 128-wide halves one
-// after the other: the promoted sums of a half are parked in shared memory (the first half in its own buffer, the second in
-// the drained stage ring), so every consumer thread holds only 64 chunk + 64 promoted accumulators.  The tensor core's fp32
+// 1 and 2 each own 64 rows of the tile and issue m64n128k16 wgmma.  The producer warpgroup lowers its register budget to 40
+// per thread and the consumer warpgroups raise theirs to 232 (setmaxnreg).  A 256-wide tile is computed as two 128-wide halves
+// one after the other: the promoted sums of a half are parked in shared memory (the first half in its own buffer, the second
+// in the drained stage ring), so every consumer thread holds 2 x 64 chunk + 64 promoted accumulators.  The tensor core's fp32
 // accumulation truncates, so K is consumed in chunks of KCH k-blocks: each chunk starts from zero in the wgmma accumulators
 // and is added to the promoted sums with one round-to-nearest FMA (which also applies the chunk's descale factor).  The
-// epilogue then works on the whole parked tile: bias, activation / ReLU mask, tile maximum, fp32 output, fp16 companion,
-// column sums.
+// tensor pipe is not drained between k-blocks: one k-block stays in flight (wait_group 1, its stage is released when the next
+// one is committed), and consecutive chunks -- across the half boundary too -- alternate between two accumulator sets, so a
+// chunk is promoted (and the first half parked) while the next chunk's MMAs run.  Summation order and roundings are those of
+// a synchronous loop, so results do not depend on the schedule.  The epilogue then works on the whole parked tile: bias,
+// activation / ReLU mask, tile maximum, fp32 output, fp16 companion, column sums.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -147,7 +151,10 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
   }
   __syncthreads();
 
+  // 384 threads x 168 registers are allocated at launch; the producer warpgroup gives 128 back per thread, the two consumer
+  // warpgroups take 64 more each: two chunk accumulator sets and the promoted sums fit (128 x 40 + 256 x 232 <= 64 K)
   if (warp < 4) {
+    setmaxnreg_dec<40>();
     // ===== TMA producer =====
     if (threadIdx.x == 0) {
       int stage = 0;
@@ -166,61 +173,35 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
       }
     }
   } else {
+    setmaxnreg_inc<232>();
     if (nkb > 0) {
       // ===== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =====
       const int tid = threadIdx.x - 128;
       const int wg = tid >> 7;
       const int wl = (tid >> 5) & 3;            // warp inside the warpgroup: fragment rows 16 wl .. 16 wl + 15
+      const bool leader = (tid & 127) == 0;     // arrives on empty[] for the warpgroup
       // A sub-tile of this warpgroup: K-major 64 rows x 64 B = 4096 B in; MN-major the second 64-wide box, also 4096 B in
       const uint32_t a_off = (uint32_t)wg * 4096u;
-      int stage = 0;
+      // The chunks of both halves form one sequence g = sub * nch + c, accumulated alternately in d0 / d1 (chunk g in d[g & 1]).
+      // One k-block stays in flight: after committing a k-block the warpgroup waits for the one before it, releases that one's
+      // stage, and -- when the new k-block opened a chunk -- promotes the previous chunk from the other buffer (parking the first
+      // half after its last chunk) while the tensor core works on the new one.  Chunk sums, promotion order and roundings are
+      // those of a fully synchronous loop; only the waits move.
+      const int nch = (nkb + KCH - 1) / KCH;    // promotion chunks per 128-column half
+      // the chunk count through an empty asm: when the compiler can see that it is even (NSUB = 2) it drops the exit after d0,
+      // and ptxas then serialises every wgmma of the loop (C7514)
+      int nchunks = NSUB * nch;
+      asm("" : "+r"(nchunks));
+      int stage = 0;                            // stage / parity of the next k-block
       uint32_t phase = 0;
-      for (int sub = 0; sub < NSUB; ++sub) {
-        const int n0 = n0t + sub * SUB_N;
-        float acc[64];
+      int held = -1;                            // stage of the k-block in flight (released after the next one is committed)
+      float cs_prev = 0.f;                      // descale of the chunk awaiting promotion
+      float acc[64], d0[64], d1[64];
 #pragma unroll
-        for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-        for (int kc = 0; kc < nkb; kc += KCH) {
-          // descale factor of this chunk: 1 / (s_a * s_b), powers of two.  Per-tensor companions: the same word every chunk;
-          // tile-scaled companions: the word of the (128-row, 256-column) tile of the operand this chunk's k-range lies in
-          const int kstart = (kb0 + kc) * BK;
-          const int ia = A_MN ? (kstart >> 7) * ep.a_sr + (m0 >> 8) * ep.a_sc : (m0 >> 7) * ep.a_sr + (kstart >> 8) * ep.a_sc;
-          const int ib = B_MN ? (kstart >> 7) * ep.b_sr + (n0 >> 8) * ep.b_sc : 0;
-          const float cs = __uint_as_float(inv_pow2_bits(scale_bits_from_amax(__ldg(ep.amax_a + ia)))) *
-                           __uint_as_float(inv_pow2_bits(scale_bits_from_amax(__ldg(ep.amax_b + ib))));
-          float d[64];
-#pragma unroll
-          for (int j = 0; j < 64; ++j) d[j] = 0.f;
-          const int kend = min(nkb, kc + KCH);
-          for (int kb = kc; kb < kend; ++kb) {
-            mbar_wait(&full[stage], phase);
-            const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
-            const uint32_t a_hi = st + a_off, a_lo = st + A_BYTES + a_off, b_hi = st + 2 * A_BYTES, b_lo = st + 2 * A_BYTES + B_BYTES;
-#pragma unroll
-            for (int j = 0; j < 64; ++j) fence_operand(d[j]);
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < BK / WG_K; ++kk) {
-              const uint64_t dah = tile_desc<A_MN>(a_hi, kk), dal = tile_desc<A_MN>(a_lo, kk);
-              const uint64_t dbh = tile_desc<B_MN>(b_hi, kk), dbl = tile_desc<B_MN>(b_lo, kk);
-              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dal, dbh, (kb > kc || kk > 0) ? 1u : 0u);
-              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbl, 1u);
-              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbh, 1u);
-            }
-            wgmma_commit();
-            wgmma_wait_all();
-#pragma unroll
-            for (int j = 0; j < 64; ++j) fence_operand(d[j]);
-            if ((tid & 127) == 0) mbar_arrive(&empty[stage]);          // this warpgroup no longer reads the slot
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          // add the finished chunk sum into the promoted accumulators (one round-to-nearest fp32 FMA each)
-#pragma unroll
-          for (int j = 0; j < 64; ++j) acc[j] = __fmaf_rn(d[j], cs, acc[j]);
-        }
-        // park the promoted sums: fragment element j of lane l in warp wl is (row 16 wl + l/4 + 8 ((j/2)&1), column 8 (j/4) + 2 (l%4) + j%2)
-        if (sub == 1) epi_sync();                // both warpgroups are done with the stage ring before it is overwritten
-        float* park = sub ? park1 : park0;
+      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+
+      // park the promoted sums: fragment element j of lane l in warp wl is (row 16 wl + l/4 + 8 ((j/2)&1), column 8 (j/4) + 2 (l%4) + j%2)
+      auto park_acc = [&](float* park) {
         const int r0 = wg * 64 + wl * 16 + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < 64; j += 4) {
@@ -228,6 +209,72 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
           *reinterpret_cast<float2*>(park + r0 * PARK_PITCH + c) = make_float2(acc[j], acc[j + 1]);
           *reinterpret_cast<float2*>(park + (r0 + 8) * PARK_PITCH + c) = make_float2(acc[j + 2], acc[j + 3]);
         }
+      };
+      // add a finished chunk sum into the promoted accumulators (one round-to-nearest fp32 FMA each)
+      auto promote = [&](float (&p)[64], float cs) {
+#pragma unroll
+        for (int j = 0; j < 64; ++j) fence_operand(p[j]);
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[j] = __fmaf_rn(p[j], cs, acc[j]);
+      };
+      // chunk g into d (its first wgmma overwrites d: scale_d = 0); p holds chunk g - 1 (still in flight when g > 0)
+      auto run_chunk = [&](float (&d)[64], float (&p)[64], int g) {
+        const int sub = (NSUB > 1 && g >= nch) ? 1 : 0;
+        const int kc = (g - sub * nch) * KCH;
+        // descale factor of this chunk: 1 / (s_a * s_b), powers of two.  Per-tensor companions: the same word every chunk;
+        // tile-scaled companions: the word of the (128-row, 256-column) tile of the operand this chunk's k-range lies in.
+        // Read here, a chunk before the promotion that uses it.
+        const int n0 = n0t + sub * SUB_N;
+        const int kstart = (kb0 + kc) * BK;
+        const int ia = A_MN ? (kstart >> 7) * ep.a_sr + (m0 >> 8) * ep.a_sc : (m0 >> 7) * ep.a_sr + (kstart >> 8) * ep.a_sc;
+        const int ib = B_MN ? (kstart >> 7) * ep.b_sr + (n0 >> 8) * ep.b_sc : 0;
+        const float cs = __uint_as_float(inv_pow2_bits(scale_bits_from_amax(__ldg(ep.amax_a + ia)))) *
+                         __uint_as_float(inv_pow2_bits(scale_bits_from_amax(__ldg(ep.amax_b + ib))));
+        const int kend = min(nkb, kc + KCH);
+        for (int kb = kc; kb < kend; ++kb) {
+          mbar_wait(&full[stage], phase);
+          const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
+          const uint32_t a_hi = st + a_off, a_lo = st + A_BYTES + a_off, b_hi = st + 2 * A_BYTES, b_lo = st + 2 * A_BYTES + B_BYTES;
+#pragma unroll
+          for (int j = 0; j < 64; ++j) fence_operand(d[j]);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < BK / WG_K; ++kk) {
+            const uint64_t dah = tile_desc<A_MN>(a_hi, kk), dal = tile_desc<A_MN>(a_lo, kk);
+            const uint64_t dbh = tile_desc<B_MN>(b_hi, kk), dbl = tile_desc<B_MN>(b_lo, kk);
+            wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dal, dbh, (kb > kc || kk > 0) ? 1u : 0u);
+            wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbl, 1u);
+            wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbh, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();                                       // the previous k-block is done ...
+          if (held >= 0 && leader) mbar_arrive(&empty[held]);    // ... and this warpgroup no longer reads its slot
+          held = stage;
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (kb == kc && g > 0) {
+            promote(p, cs_prev);
+            if (NSUB > 1 && g == nch) {                          // chunk g - 1 was the last of the first half
+              park_acc(park0);
+#pragma unroll
+              for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+            }
+          }
+        }
+        cs_prev = cs;
+      };
+      // the last chunk, in d: drain, release the last stage, promote, park
+      auto finish = [&](float (&d)[64]) {
+        wgmma_wait<0>();
+        if (leader) mbar_arrive(&empty[held]);
+        promote(d, cs_prev);
+        if (NSUB > 1) epi_sync();                // both warpgroups are done with the stage ring before it is overwritten
+        park_acc(NSUB > 1 ? park1 : park0);
+      };
+      for (int g = 0;; g += 2) {                 // unrolled by two: d0 / d1 are indexed at compile time
+        run_chunk(d0, d1, g);
+        if (g + 1 == nchunks) { finish(d0); break; }
+        run_chunk(d1, d0, g + 1);
+        if (g + 2 == nchunks) { finish(d1); break; }
       }
       epi_sync();
 

@@ -51,9 +51,18 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 // ---- warpgroup MMA ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// waits until at most N committed wgmma groups of this warp are still pending
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accesses of an accumulator register across the asynchronous MMAs
 __device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// per-thread register budget of the executing warpgroup (all 128 threads execute it): dec gives registers back to the CTA's pool,
+// inc takes them from it (blocking until they are free)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // D[64 x 128] (+)= A[64 x 16] * B[16 x 128], fp16 operands from shared memory, fp32 accumulators in registers.
 // TA / TB = 1: the operand is MN-major in shared memory (transposed), 0: K-major.  scale_d = 0 overwrites D.
