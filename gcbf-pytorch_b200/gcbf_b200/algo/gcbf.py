@@ -10,6 +10,7 @@ What changes relative to the reference's `update` body (results identical, see t
     global-norm clip + Adam as one fused kernel per net (gcbf.py:220-226);
   * the M x M broadcast of `acc/derivative` (gcbf.py:209) is an exact pair count, not an M x M temporary.
 """
+import ctypes
 import os
 from typing import Dict, List, Optional
 
@@ -731,6 +732,163 @@ class GCBF(Algorithm):
         native.check(native.fn('gcbf_cbf_field_probe_fill')(ctypes.byref(d), rowptr.data_ptr(), ei.data_ptr() if E else None, E,
                                                             ea.data_ptr() if E else None, _C.stream()), 'gcbf_cbf_field_probe_fill')
         return ei, ea
+
+    # ---- CBF-condition field: where the learned controller keeps h_dot + alpha h >= 0 ---------------------------------------------
+    COND_MAX_PROBES = 65536             # default probe bound of one chunk
+    COND_MAX_EDGES = 262144             # default two-hop edge bound of one chunk (actor and CBF passes over at most this many edges)
+
+    def cbf_condition_field(self, data, agents=0, x_dim: int = 0, y_dim: int = 1, n_mesh: int = 30, lims=None, relink: bool = False,
+                            max_probes: Optional[int] = None, max_edges: Optional[int] = None):
+        """h and h_dot of the given agents over the grid of cbf_field, under the learned controller: for graph b, agent a = agents[k]
+        and grid point (i, j), G' is graph b alone with s_a[x_dim] = xs[j], s_a[y_dim] = ys[i] (edges kept with edge_attr recomputed,
+        or with relink=True the radius graph of the moved states), u = actor(G') with u_ref(G') as its head input, x_dot = f(s,
+        clamp(u + u_ref)) with the single-graph reach-freeze, and (h, h_dot) = h_dot_analytic(G', u, freeze=True) at row a: h_dot with
+        the edges of G' held fixed.  Goals: data.goal of graph b if present, else env._goal.  The CBF condition h_dot + alpha h >= 0
+        certifies safety where it holds.
+
+        Returns (xs, ys, h, h_dot), the fields [B, A, n_mesh, n_mesh] in cbf_field's index order.  Instead of n_mesh^2 copies per agent,
+        each grid point is a two-hop probe graph (gcbf_cbf_condition_probe_count / _fill, csrc/condition.cu): the moved agent a' and
+        one row j' per agent neighbour j, whose actions the derivative needs.  A call advances the spectral-norm vectors of the actor and
+        of the CBF by ONE power iteration each and uses that 1/sigma in every chunk of at most max_probes probes / max_edges two-hop
+        edges; one host sync per call (the per-probe counts).  The chunk count and the two-hop edges go to self.last_field_chunks /
+        self.last_field_edges."""
+        d, keep, xs, ys, B, A, T, plan = self._condition_plan(data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges)
+        from .. import jvp
+        env = self._env
+        dev = data.states.device
+        actor_spec = self.actor.feat_transformer.module_0.net_spec(self.actor.feat_2_action)
+        cbf_spec = self.cbf.feat_transformer.module_0.net_spec(self.cbf.feat_2_CBF)
+        h = torch.empty(T, device=dev, dtype=torch.float32)
+        h_dot = torch.empty(T, device=dev, dtype=torch.float32)
+        edges = 0
+        with torch.no_grad():
+            sig_actor = ops.sn_power_iter_batched(actor_spec.all_layers())     # ONE power iteration per net for the whole call
+            sig_cbf = ops.sn_power_iter_batched(cbf_spec.all_layers())
+            for t0, t1, Ea, Rc, Ec, off in plan['chunks']:
+                ck = self._condition_fill(d, keep, plan, t0, t1, Rc, Ec, off, rows=False)
+                xb, st, gl, ei, ea, NN = ck['x'], ck['states'], ck['goal'], ck['edge_index'], ck['edge_attr'], ck['num_rows']
+                rowptr = ops.rowptr_from_edge_index(ei, NN, check_sorted=False)
+                rows = torch.arange(Rc, device=dev, dtype=torch.int64)
+                # per-row closed loop: every a' / j' row is a graph of one agent with its own goal (bit for bit the per-graph kernels)
+                cfg1 = self._row_cfg(Rc, 1)
+                uref = torch.empty(Rc, env.action_dim, device=dev, dtype=torch.float32)
+                _C.call('gcbf_u_ref_multi', ctypes.byref(cfg1), _C.ptr(st), env.state_dim, _C.ptr(gl), plan['goal_dim'],
+                        _C.ptr(env._gain()), _C.ptr(uref))
+                u, _ = ops.net_forward(actor_spec, xb, ea, ei, rowptr, rows, uref, False, sigma=sig_actor)
+                sdot = torch.empty(NN, env.state_dim, device=dev, dtype=torch.float32)
+                _C.call('gcbf_state_dot', ctypes.byref(cfg1), _C.ptr(st), env.state_dim, _C.ptr(u), _C.ptr(uref), _C.ptr(gl),
+                        plan['goal_dim'], 1, 1, _C.ptr(sdot), env.state_dim)
+                # the original rows are read as obstacle sources of a' only: x_dot of a node without an action
+                cfg0 = self._row_cfg(B, 0)
+                _C.call('gcbf_state_dot', ctypes.byref(cfg0), _C.ptr(st[Rc:]), env.state_dim, None, None, None, 0, 0, 0,
+                        _C.ptr(sdot[Rc:]), env.state_dim)
+                # the CBF over the a' rows and their edges (the first Ea: edges are target-sorted, a' rows first)
+                ei_a = ei[:, :Ea].contiguous()
+                rowptr_a = ops.rowptr_from_edge_index(ei_a, NN, check_sorted=False)
+                h_c, ctx = ops.net_forward(cbf_spec, xb, ea[:Ea], ei_a, rowptr_a, rows[:t1 - t0], None, True, sigma=sig_cbf)
+                t_ea = jvp.edge_attr_tangent(env, st, sdot, ei_a)
+                hd_c = jvp.net_tangent(cbf_spec, ctx, t_ea, rowptr_a, rows[:t1 - t0])
+                h[t0:t1].copy_(h_c.view(-1))
+                h_dot[t0:t1].copy_(hd_c.view(-1))
+                edges += Ec
+        self.last_field_chunks, self.last_field_edges = len(plan['chunks']), edges
+        shape = (B, A, int(n_mesh), int(n_mesh))
+        return xs, ys, h.view(shape), h_dot.view(shape)
+
+    def cbf_condition_field_probe_graph(self, data, agents=0, x_dim: int = 0, y_dim: int = 1, n_mesh: int = 30, lims=None,
+                                        relink: bool = False) -> dict:
+        """The two-hop probe graphs cbf_condition_field feeds the nets, all probes as one chunk, for inspection: 'rows' [R, 3] int64 =
+        (kind 0 a' / 1 j', node id in `data`, probe id) of the probe rows, 'edge_index' [2, E] over rows (a source >= R is the original
+        node source - R), target-sorted with the a' rows first, 'edge_attr' [E, edge_dim] = g(s_src) - g(s_tgt) in G', 'states' [R,
+        state_dim] and 'goal' [R, goal_dim] of the rows.  Same arguments as cbf_condition_field; no net is evaluated (u, v unchanged)."""
+        d, keep, xs, ys, B, A, T, plan = self._condition_plan(data, agents, x_dim, y_dim, n_mesh, lims, relink, None, None,
+                                                              one_chunk=True)
+        t0, t1, Ea, Rc, Ec, off = plan['chunks'][0]
+        ck = self._condition_fill(d, keep, plan, t0, t1, Rc, Ec, off, rows=True)
+        return dict(rows=ck['rows'], edge_index=ck['edge_index'], edge_attr=ck['edge_attr'], states=ck['states'][:Rc],
+                    goal=ck['goal'], num_moved_edges=Ea)
+
+    def _row_cfg(self, num_graphs: int, num_agents: int):
+        """gcbf_env_cfg of num_graphs graphs of max(num_agents, 1) nodes: the per-row closed loop of the condition field."""
+        cfg = self._env._cfg(num_graphs)
+        if num_agents == 1:
+            cfg.nodes_per_graph, cfg.num_agents = 1, 1
+        else:
+            cfg.num_agents = 0
+        return cfg
+
+    def _condition_plan(self, data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges, one_chunk: bool = False):
+        """Argument checks (all before any launch), the per-probe counts (the call's one host sync) and the chunks: (desc, tensors it
+        points into, xs, ys, B, A, T, plan)."""
+        if max_probes is not None and int(max_probes) < 1:
+            raise ValueError(f'max_probes must be >= 1, got {max_probes}')
+        if max_edges is not None and not 1 <= int(max_edges) < 2 ** 31:
+            raise ValueError(f'max_edges must be in [1, 2^31), got {max_edges}')
+        d, keep, xs, ys, B, A, T = self._field_desc(data, agents, x_dim, y_dim, n_mesh, lims, relink, None, None)
+        env = self._env
+        dev = data.states.device
+        goal_pg = getattr(data, 'goal', None) if hasattr(data, 'goal') else None
+        goals = (goal_pg if goal_pg is not None else env._goal)
+        if goals is None:
+            raise RuntimeError('cbf_condition_field needs the goals (data.goal or env._goal: reset() or set_goal() first)')
+        goals = goals.detach().to(dev, torch.float32).contiguous()
+        gd = min(int(goals.shape[1]), 6)
+        counts = torch.empty(3, T, device=dev, dtype=torch.int32)
+        _C.call('gcbf_cbf_condition_probe_count', ctypes.byref(d), _C.ptr(counts))
+        c = counts.cpu().numpy().astype(np.int64)                      # the call's one host sync
+        ea, nj, ej = c[0], c[1], c[2]
+        e_all = ea + ej
+        BN = B * env.nodes_per_graph
+        P = T if one_chunk else min(T, int(max_probes) if max_probes is not None else self.COND_MAX_PROBES)
+        Emax = 2 ** 31 - 1 if one_chunk else (int(max_edges) if max_edges is not None else self.COND_MAX_EDGES)
+        big = int(e_all.max()) if T else 0
+        if big > Emax:
+            raise ValueError(f'a probe has {big} two-hop edges > max_edges {Emax}')
+        cum = np.concatenate([[0], np.cumsum(e_all)])
+        chunks, offs = [], []
+        t0, pos = 0, 0
+        while t0 < T:
+            t1 = min(t0 + P, int(np.searchsorted(cum, cum[t0] + Emax, side='right')) - 1)
+            sl = slice(t0, t1)
+            Ea, Rc = int(ea[sl].sum()), (t1 - t0) + int(nj[sl].sum())
+            Ec = Ea + int(ej[sl].sum())
+            if Ec >= 2 ** 31 or Rc + BN >= 2 ** 31:
+                raise ValueError(f'probes [{t0}, {t1}): {Rc} rows / {Ec} edges overflow int32; lower max_probes / max_edges')
+            excl = lambda v, start: start + np.concatenate([[0], np.cumsum(v)[:-1]])
+            offs.append(np.concatenate([excl(ea[sl], 0), excl(nj[sl], t1 - t0), excl(ej[sl], Ea)]))
+            chunks.append((t0, t1, Ea, Rc, Ec, (pos, 3 * (t1 - t0))))
+            pos += 3 * (t1 - t0)
+            t0 = t1
+        host = torch.from_numpy(np.concatenate(offs).astype(np.int32))
+        if torch.cuda.is_available():
+            host = host.pin_memory()
+        off_dev = host.to(dev, non_blocking=True)                       # every chunk's offsets in one copy, no second sync
+        plan = dict(chunks=chunks, offsets=off_dev, goals=goals, goal_dim=gd, goal_per_graph=goal_pg is not None, BN=BN,
+                    counts=counts)
+        return d, keep, xs, ys, B, A, T, plan
+
+    def _condition_fill(self, d, keep, plan, t0, t1, Rc, Ec, off, rows: bool) -> dict:
+        """Rows [0, Rc) and the Ec edges of probes [t0, t1), followed by the original rows (gcbf_cbf_condition_probe_fill)."""
+        env = self._env
+        st0, x0 = keep[0], keep[1]
+        dev = x0.device
+        BN, gd, goals = plan['BN'], plan['goal_dim'], plan['goals']
+        NN = Rc + BN
+        nd, sd = int(x0.shape[1]), env.state_dim
+        xb = torch.empty(NN, nd, device=dev, dtype=torch.float32)
+        xb[Rc:].copy_(x0)
+        st = torch.empty(NN, sd, device=dev, dtype=torch.float32)
+        st[Rc:].copy_(st0[:, :sd])
+        gl = torch.empty(Rc, gd, device=dev, dtype=torch.float32)
+        rw = torch.empty(Rc, 3, device=dev, dtype=torch.int64) if rows else None
+        ei = torch.empty(2, Ec, device=dev, dtype=torch.int64)
+        ea = torch.empty(Ec, env.edge_dim, device=dev, dtype=torch.float32)
+        o0, _ = off
+        offp = plan['offsets'].data_ptr() + 4 * o0
+        _C.call('gcbf_cbf_condition_probe_fill', ctypes.byref(d), _C.ptr(goals), int(goals.shape[1]), gd, 1 if plan['goal_per_graph'] else 0,
+                t0, t1 - t0, offp, Rc, _C.ptr(xb), _C.ptr(st), _C.ptr(gl), _C.ptr(rw), _C.ptr(ei) if Ec else None, Ec,
+                _C.ptr(ea) if Ec else None)
+        return dict(x=xb, states=st, goal=gl, rows=rw, edge_index=ei, edge_attr=ea, num_rows=NN)
 
     def _field_desc(self, data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges):
         """Argument checks (all before any launch) and the gcbf_field_desc of a field call: (desc, tensors it points into + the CBF's

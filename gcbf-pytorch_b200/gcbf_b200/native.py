@@ -110,6 +110,9 @@ SIGS = {
     'gcbf_cbf_field': (c_int, [POINTER(FieldDesc), P, POINTER(c_int64), P, c_size_t, P]),
     'gcbf_cbf_field_probe_count': (c_int, [POINTER(FieldDesc), P, P]),
     'gcbf_cbf_field_probe_fill': (c_int, [POINTER(FieldDesc), P, P, c_int64, P, P]),
+    'gcbf_cbf_condition_probe_count': (c_int, [POINTER(FieldDesc), P, P]),
+    'gcbf_cbf_condition_probe_fill': (c_int, [POINTER(FieldDesc), P, c_int, c_int, c_int, c_int64, c_int, P, c_int64, P, P, P, P, P, c_int64,
+                                              P, P]),
     'gcbf_linear_fwd_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P]),
     'gcbf_linear_bwd_data_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
                                        c_int, c_int, c_int, P]),

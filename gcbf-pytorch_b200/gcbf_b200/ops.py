@@ -911,9 +911,10 @@ class NetSpec:
         return self.phi + self.gate + self.gamma + (self.head or [])
 
 
-def net_forward(spec: NetSpec, x, edge_attr, edge_index, rowptr, row_index, head_extra, save):
+def net_forward(spec: NetSpec, x, edge_attr, edge_index, rowptr, row_index, head_extra, save, sigma=None):
     """phi -> attention aggregation -> gamma (on `row_index` rows only when given) -> head.
-    Returns (out, ctx-tuple)."""
+    Returns (out, ctx-tuple).  sigma: (inv_sigmas, uvs) of an earlier sn_power_iter_batched(spec.all_layers()) to use instead of a
+    new power iteration (passes that share one spectral-norm step, e.g. the chunks of one field call)."""
     dev = x.device
     E = edge_index.shape[1]
     Nn = x.shape[0]
@@ -926,7 +927,7 @@ def net_forward(spec: NetSpec, x, edge_attr, edge_index, rowptr, row_index, head
          E, ptr(ein) if E else None, kin)
     # the power iterations depend on the weights only: all spectral-normalised layers of the net in one batched call
     n_phi, n_gate, n_gamma = len(spec.phi), len(spec.gate), len(spec.gamma)
-    isg, uvs = sn_power_iter_batched(spec.all_layers(), snapshot=save)
+    isg, uvs = sn_power_iter_batched(spec.all_layers(), snapshot=save) if sigma is None else sigma
     R = row_index.numel() if row_index is not None else Nn
     prepare_weights([(L, E) for L in spec.phi + spec.gate] + [(L, R) for L in spec.gamma + (spec.head or [])])
     isg_phi, isg_gate = isg[:n_phi], isg[n_phi:n_phi + n_gate]

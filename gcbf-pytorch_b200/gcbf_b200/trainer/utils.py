@@ -53,14 +53,24 @@ def init_logger(log_path: str, env: str, algo: str, seed: int, args: dict = None
     return run
 
 
-def cbf_contour_data(cbf_algo, data, env, agent_id: int, x_dim: int, y_dim: int, attention: bool = True, n_mesh: int = 30) -> dict:
+def cbf_contour_data(cbf_algo, data, env, agent_id: int, x_dim: int, y_dim: int, attention: bool = True, n_mesh: int = 30,
+                     condition: bool = False) -> dict:
     """What the reference's plot_cbf_contour (gcbf/trainer/utils.py:226-298) plots, without plotting: the meshgrids `x`, `y`
     [n_mesh, n_mesh] of env.state_lim along (x_dim, y_dim), the learned CBF `cbf` [n_mesh, n_mesh] of agent `agent_id` on them
     (cbf[i, j] at (x[i, j], y[i, j]); GCBF.cbf_field, one library call) and, with `attention`, the attention weights [E, 1] of
-    `data` (cbf.attention, utils.py:292-293).  Its zero level set is the learned safe-set boundary."""
-    xs, ys, h = cbf_algo.cbf_field(data, agents=int(agent_id), x_dim=x_dim, y_dim=y_dim, n_mesh=n_mesh, lims=env.state_lim)
+    `data` (cbf.attention, utils.py:292-293).  Its zero level set is the learned safe-set boundary.  With `condition`, also
+    `h_dot` and `condition` = h_dot + alpha * cbf [n_mesh, n_mesh] under the learned controller (GCBF.cbf_condition_field; alpha =
+    cbf_algo.params['alpha']): the certificate holds where condition >= 0."""
+    if condition:
+        xs, ys, h, h_dot = cbf_algo.cbf_condition_field(data, agents=int(agent_id), x_dim=x_dim, y_dim=y_dim, n_mesh=n_mesh,
+                                                        lims=env.state_lim)
+    else:
+        xs, ys, h = cbf_algo.cbf_field(data, agents=int(agent_id), x_dim=x_dim, y_dim=y_dim, n_mesh=n_mesh, lims=env.state_lim)
     x, y = np.meshgrid(xs, ys)
     out = dict(x=x, y=y, cbf=h[0, 0].detach().cpu())
+    if condition:
+        out['h_dot'] = h_dot[0, 0].detach().cpu()
+        out['condition'] = out['h_dot'] + float(cbf_algo.params['alpha']) * out['cbf']
     if attention:
         out['attention'] = cbf_algo.cbf.attention(data)
     return out

@@ -497,6 +497,30 @@ int gcbf_cbf_field_probe_count(const gcbf_field_desc* d, int32_t* rowptr, void* 
 int gcbf_cbf_field_probe_fill(const gcbf_field_desc* d, const int32_t* rowptr, int64_t* edge_index, int64_t num_edges, float* edge_attr,
                               void* stream);
 
+/* CBF-condition field: two-hop probe graphs.  For probe t (numbered as above: graph b's agent a moved to s'_t), G' is graph b with a
+ * at s'_t: its given edges with edge_attr recomputed (relink == 0), or the K1 radius graph of its states (relink != 0).  The field is
+ * h and h_dot = sum over a's in-edges of dh_a/de . (g_dot(s_src) - g_dot(s'_a)) of agent a in G' under the learned controller,
+ * x_dot = f(s, clamp(u + u_ref(s))) with u = actor(G') and the single-graph reach-freeze; h_dot needs x_dot at a and at every agent
+ * source j of a, and u_j reads j's own in-edges in G'.  So each probe becomes these rows:
+ *   a'  the moved agent, with a's in-edges in G';
+ *   j'  one row per agent source j of a', in a'-edge order: j's unmoved state, with j's in-edges in G' (fixed: j's in-edges in the
+ *       given graph; relink: every node k != j of graph b inside the radius of s_j, ascending k), where the source a is the a' row;
+ * and a''s in-edges from agent j point at the j' rows.  Obstacle sources, and every other source of a j' row, point at the original
+ * node's row src_off + node id.  Every target's edges keep the copy's order (ascending original source id, or the given order).
+ * d->cbf is read for node_dim only; d->x is required (the x rows); the chunk bounds are not read.
+ * count writes counts [3, T] int32 (T = num_graphs * num_probe_agents * ny * nx): a' in-edges, j' rows, in-edges of all j' rows.
+ * fill builds probes [t0, t0 + num_probes) given offsets [3, num_probes] int32 (exclusive scans over these probes of the three
+ * counts, the j' row offsets plus num_probes, the j' edge offsets plus the chunk's a' edge total: edges are target-sorted, a' rows
+ * first).  It writes per row r: x_out [r, node_dim], states_out [r, state_dim] (the state in G'), goal_out [r, goal_dim] (the row's
+ * goal: goal row of (b, agent) in a [num_agents, ld_goal] set, or one set per graph with goal_per_graph), rows_out [r, 3] int64
+ * (optional: kind 0 a' / 1 j', original node id, probe id); edge_index [2, num_edges] (target rows) and edge_attr [num_edges,
+ * edge_dim] = g(s_src) - g(s_tgt) in G'.  Preconditions not checked on the device: agent ids in [0, num_agents), offsets consistent
+ * with count, the given graph's edge_index target-sorted inside its graphs with rowptr its CSR (fixed mode). */
+int gcbf_cbf_condition_probe_count(const gcbf_field_desc* d, int32_t* counts, void* stream);
+int gcbf_cbf_condition_probe_fill(const gcbf_field_desc* d, const float* goal, int ld_goal, int goal_dim, int goal_per_graph, int64_t t0,
+                                  int num_probes, const int32_t* offsets, int64_t src_off, float* x_out, float* states_out, float* goal_out,
+                                  int64_t* rows_out, int64_t* edge_index, int64_t num_edges, float* edge_attr, void* stream);
+
 /* Batched episode reset of a vectorised rollout (num_envs copies of one env, nodes_per_graph = num_agents + num_obs rows each, agents
  * first): in ONE launch, every env e that is done -- step_count[e] >= max_steps, or (reach != NULL) all reach[e * num_agents + i] set,
  * the reference's `done` of env.step -- is re-sampled in place with the algorithm of that env's reset() (gcbf/env/<env>.py):
