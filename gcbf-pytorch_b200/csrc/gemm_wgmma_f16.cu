@@ -33,6 +33,8 @@
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
+#include <atomic>
+
 #include "common.cuh"
 #include "sm90_ptx.cuh"
 
@@ -49,14 +51,19 @@ constexpr int NUM_THREADS = 384;       // warpgroup 0: TMA producer (one thread)
 constexpr int EPI_THREADS = 256;
 constexpr int KCH_MAX = 256 / BK;      // k-blocks accumulated inside the tensor core before promotion to registers: upper limit (256 K-elements)
 constexpr int MN_BOX = 64;             // MN-major operands: one TMA box = 64 MN elements (128 B, SWIZZLE_128B) x BK k-rows
-constexpr int STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2;                         // one of hi / lo
 constexpr int B_BYTES = SUB_N * BK * 2;
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;       // 32 KB
+constexpr int RING_BYTES = 128 * 1024;                       // the stage ring, the same size for both product counts
+// Products per k-slice P: 3 = hi*hi + lo*hi + hi*lo (fp32-grade, the default), 1 = hi*hi only (fp16 operands).  A P = 1 stage holds
+// only the hi planes (16 KB), so the same ring is 8 stages deep instead of 4: a k-block has a third of the MMAs of a P = 3 one and
+// half its bytes, and the deeper ring keeps twice as many k-blocks of loads in flight to feed it.
+template <int P> __host__ __device__ constexpr int stage_bytes() { return P == 3 ? 2 * A_BYTES + 2 * B_BYTES : A_BYTES + B_BYTES; }   // 32 / 16 KB
+template <int P> __host__ __device__ constexpr int stages() { return RING_BYTES / stage_bytes<P>(); }                                // 4 / 8
 constexpr int PARK_PITCH = SUB_N + 8;                        // floats; conflict-free float2 stores of the accumulator fragments
 constexpr int PARK_BYTES = BM * PARK_PITCH * 4;
-static_assert(PARK_BYTES <= STAGES * STAGE_BYTES, "the second half of a 256-wide tile is parked in the stage ring");
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + PARK_BYTES + 1024 /*align slack*/ + 256 /*barriers, reductions*/;
+static_assert(PARK_BYTES <= RING_BYTES, "the second half of a 256-wide tile is parked in the stage ring");
+static_assert(2 * stages<1>() * 8 + (256 / 32) * 4 <= 256, "barriers and reduction words fit their 256 bytes");
+constexpr int SMEM_BYTES = RING_BYTES + PARK_BYTES + 1024 /*align slack*/ + 256 /*barriers, reductions*/;
 
 enum { EPI_FWD = 0, EPI_DGRAD = 1, EPI_WGRAD = 2 };
 
@@ -118,19 +125,23 @@ __device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* map, 
 
 __device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory"); }
 
-// grid (tiles_m * tiles_n, contraction splits)
-template <int BN, bool A_MN, bool B_MN>
+// grid (tiles_m * tiles_n, contraction splits).  P = 1: the lo maps are not read (the launcher passes the hi maps in their place).
+template <int BN, bool A_MN, bool B_MN, int P>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
               const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
               float* __restrict__ C, int ldc, int Mo, int No, int tiles_n, int kblocks_per_split, int kblocks_total, int KCH, EpiParams ep) {
+  static_assert(P == 3 || P == 1, "products per k-slice: 3 (3xFP16) or 1 (fp16)");
+  constexpr int STAGES = stages<P>();
+  constexpr int STAGE_BYTES = stage_bytes<P>();
+  constexpr int B_OFF = (P == 3 ? 2 : 1) * A_BYTES;       // stage layout: [A hi][A lo][B hi][B lo], or [A hi][B hi]
   constexpr int NSUB = BN / SUB_N;
   constexpr int MODE = A_MN ? EPI_WGRAD : (B_MN ? EPI_DGRAD : EPI_FWD);   // the operand layouts identify the product
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* park0 = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // columns [0, 128) of the tile
+  float* park0 = reinterpret_cast<float*>(smem + RING_BYTES);            // columns [0, 128) of the tile
   float* park1 = reinterpret_cast<float*>(smem);                          // columns [128, 256): the drained stage ring
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + PARK_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_BYTES + PARK_BYTES);
   uint64_t* full = bars;                        // [STAGES]  TMA -> MMA
   uint64_t* empty = bars + STAGES;              // [STAGES]  MMA -> TMA (one arrive per consumer warpgroup)
   uint32_t* red = reinterpret_cast<uint32_t*>(bars + 2 * STAGES);   // [EPI_THREADS / 32] per-warp maxima
@@ -143,9 +154,9 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a_hi);
-    tma_prefetch_desc(&map_a_lo);
+    if (P == 3) tma_prefetch_desc(&map_a_lo);
     tma_prefetch_desc(&map_b_hi);
-    tma_prefetch_desc(&map_b_lo);
+    if (P == 3) tma_prefetch_desc(&map_b_lo);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_barrier_init();
   }
@@ -165,9 +176,9 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
           uint8_t* st = smem + stage * STAGE_BYTES;
           mbar_expect_tx(&full[stage], STAGE_BYTES);
           load_tile<A_MN>(st, &map_a_hi, &full[stage], m0, kb * BK, BM);
-          load_tile<A_MN>(st + A_BYTES, &map_a_lo, &full[stage], m0, kb * BK, BM);
-          load_tile<B_MN>(st + 2 * A_BYTES, &map_b_hi, &full[stage], n0t + sub * SUB_N, kb * BK, SUB_N);
-          load_tile<B_MN>(st + 2 * A_BYTES + B_BYTES, &map_b_lo, &full[stage], n0t + sub * SUB_N, kb * BK, SUB_N);
+          if (P == 3) load_tile<A_MN>(st + A_BYTES, &map_a_lo, &full[stage], m0, kb * BK, BM);
+          load_tile<B_MN>(st + B_OFF, &map_b_hi, &full[stage], n0t + sub * SUB_N, kb * BK, SUB_N);
+          if (P == 3) load_tile<B_MN>(st + B_OFF + B_BYTES, &map_b_lo, &full[stage], n0t + sub * SUB_N, kb * BK, SUB_N);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -234,17 +245,22 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
         for (int kb = kc; kb < kend; ++kb) {
           mbar_wait(&full[stage], phase);
           const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
-          const uint32_t a_hi = st + a_off, a_lo = st + A_BYTES + a_off, b_hi = st + 2 * A_BYTES, b_lo = st + 2 * A_BYTES + B_BYTES;
+          const uint32_t a_hi = st + a_off, a_lo = st + A_BYTES + a_off, b_hi = st + B_OFF, b_lo = st + B_OFF + B_BYTES;
 #pragma unroll
           for (int j = 0; j < 64; ++j) fence_operand(d[j]);
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < BK / WG_K; ++kk) {
-            const uint64_t dah = tile_desc<A_MN>(a_hi, kk), dal = tile_desc<A_MN>(a_lo, kk);
-            const uint64_t dbh = tile_desc<B_MN>(b_hi, kk), dbl = tile_desc<B_MN>(b_lo, kk);
-            wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dal, dbh, (kb > kc || kk > 0) ? 1u : 0u);
-            wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbl, 1u);
-            wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbh, 1u);
+            if constexpr (P == 3) {
+              const uint64_t dah = tile_desc<A_MN>(a_hi, kk), dal = tile_desc<A_MN>(a_lo, kk);
+              const uint64_t dbh = tile_desc<B_MN>(b_hi, kk), dbl = tile_desc<B_MN>(b_lo, kk);
+              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dal, dbh, (kb > kc || kk > 0) ? 1u : 0u);
+              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbl, 1u);
+              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbh, 1u);
+            } else {
+              const uint64_t dah = tile_desc<A_MN>(a_hi, kk), dbh = tile_desc<B_MN>(b_hi, kk);
+              wgmma_m64n128k16_f16<A_MN ? 1 : 0, B_MN ? 1 : 0>(d, dah, dbh, (kb > kc || kk > 0) ? 1u : 0u);
+            }
           }
           wgmma_commit();
           wgmma_wait<1>();                                       // the previous k-block is done ...
@@ -622,6 +638,9 @@ static int make_map(CUtensorMap* map, const __half* base, int rows, int cols, in
   return GCBF_OK;
 }
 
+// wgmma launches per product count ([0]: 3xFP16, [1]: one product), read by gcbf_tc_launch_count: which kernels a pass really ran
+static std::atomic<long long> g_tc_launches[2];
+
 static bool g_env_read = false;
 // k-blocks per promotion chunk.  The tensor core TRUNCATES its fp32 accumulator on every MMA (tools/acc_probe.py): the bias grows with the
 // number of MMAs accumulated before the chunk sum is promoted to registers with round-to-nearest.  4 k-blocks = 128 K-elements = 24 MMAs
@@ -641,7 +660,7 @@ struct OutH {
   __half* hi; int rows; int cols; int ld_h; uint32_t* tile_amax; int amax_stride;
 };
 
-template <int BN, bool A_MN, bool B_MN>
+template <int BN, bool A_MN, bool B_MN, int P>
 static int launch(const Operand& A, const Operand& B, float* C, int ldc, int Mo, int No, int Kc, int splits, EpiParams ep,
                   const OutH* oh, cudaStream_t st) {
   if (!g_env_read) {
@@ -658,15 +677,19 @@ static int launch(const Operand& A, const Operand& B, float* C, int ldc, int Mo,
   }
   CUtensorMap mah, mal, mbh, mbl;
   if (int rc = make_map(&mah, A.hi, A.rows, A.cols, A.ld_h, A_MN, BM)) return rc;
-  if (int rc = make_map(&mal, A.lo(), A.rows, A.cols, A.ld_h, A_MN, BM)) return rc;
   if (int rc = make_map(&mbh, B.hi, B.rows, B.cols, B.ld_h, B_MN, SUB_N)) return rc;
-  if (int rc = make_map(&mbl, B.lo(), B.rows, B.cols, B.ld_h, B_MN, SUB_N)) return rc;
+  if (P == 3) {
+    if (int rc = make_map(&mal, A.lo(), A.rows, A.cols, A.ld_h, A_MN, BM)) return rc;
+    if (int rc = make_map(&mbl, B.lo(), B.rows, B.cols, B.ld_h, B_MN, SUB_N)) return rc;
+  } else {
+    mal = mah; mbl = mbh;                   // not read by the one-product kernel
+  }
   if (oh) {
     ep.out_h = oh->hi; ep.ld_out_h = oh->ld_h; ep.out_tile_amax = oh->tile_amax; ep.out_amax_stride = oh->amax_stride;
   }
   static bool attr_set = false;
   if (!attr_set) {
-    GCBF_CUDA_OK(cudaFuncSetAttribute(gemm_h_kernel<BN, A_MN, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    GCBF_CUDA_OK(cudaFuncSetAttribute(gemm_h_kernel<BN, A_MN, B_MN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     attr_set = true;
   }
   const int tiles_m = ceil_div(Mo, BM), tiles_n = ceil_div(No, BN);
@@ -691,10 +714,11 @@ static int launch(const Operand& A, const Operand& B, float* C, int ldc, int Mo,
     GCBF_CUDA_OK(scratch_alloc((void**)&colsum_part, (size_t)tiles_m * No * 4, st));
     ep.colsum = colsum_part;
   }
-  gemm_h_kernel<BN, A_MN, B_MN><<<dim3(tiles_m * tiles_n, nsplit), NUM_THREADS, SMEM_BYTES, st>>>(mah, mal, mbh, mbl, part ? part : C,
-                                                                                                 part ? No : ldc, Mo, No, tiles_n, kps,
-                                                                                                 kblocks, kch, ep);
+  gemm_h_kernel<BN, A_MN, B_MN, P><<<dim3(tiles_m * tiles_n, nsplit), NUM_THREADS, SMEM_BYTES, st>>>(mah, mal, mbh, mbl, part ? part : C,
+                                                                                                    part ? No : ldc, Mo, No, tiles_n, kps,
+                                                                                                    kblocks, kch, ep);
   GCBF_LAUNCH_OK();
+  g_tc_launches[P == 1 ? 1 : 0].fetch_add(1, std::memory_order_relaxed);
   if (part) {
     GCBF_CUDA_OK(add_partials(part, nsplit, Mo, No, C, ldc, accumulate, st));
     GCBF_CUDA_OK(scratch_free(part, st));
@@ -704,6 +728,14 @@ static int launch(const Operand& A, const Operand& B, float* C, int ldc, int Mo,
     GCBF_CUDA_OK(scratch_free(colsum_part, st));
   }
   return GCBF_OK;
+}
+
+// products per k-slice chosen at run time: 3 (3xFP16) or 1 (fp16 operands, the hi planes only)
+template <int BN, bool A_MN, bool B_MN>
+static int launch_p(int products, const Operand& A, const Operand& B, float* C, int ldc, int Mo, int No, int Kc, int splits,
+                    const EpiParams& ep, const OutH* oh, cudaStream_t st) {
+  return products == 1 ? launch<BN, A_MN, B_MN, 1>(A, B, C, ldc, Mo, No, Kc, splits, ep, oh, st)
+                       : launch<BN, A_MN, B_MN, 3>(A, B, C, ldc, Mo, No, Kc, splits, ep, oh, st);
 }
 
 static int check_plane(const void* p, int ld_h, const char* what) {
@@ -791,6 +823,12 @@ extern "C" int gcbf_amax_split_batched(const gcbf_split_desc* descs, int count, 
   return GCBF_OK;
 }
 
+extern "C" long long gcbf_tc_launch_count(int products, int reset) {
+  if (products != 1 && products != 3) { set_error("gcbf_tc_launch_count: products %d (3 or 1)", products); return -1; }
+  std::atomic<long long>& c = th::g_tc_launches[products == 1 ? 1 : 0];
+  return reset ? c.exchange(0) : c.load();
+}
+
 extern "C" int gcbf_linear_h_supported(int M, int N, int K) {
   // the rule the host mirror applies per layer (forward, data-grad and weight-grad alike): enough rows to fill 128-row tiles,
   // both feature dimensions wide enough to be a tile / a contraction, and enough work to amortise the split pass
@@ -805,10 +843,12 @@ static int check_h16(const gcbf_h16* h, const char* what, int rows, int cols) {
   return th::check_plane(h->buf, h->ld, what);
 }
 
-// Y[M,N] = act(alpha * X W^T + bias): A = X companion [M][K] (K-major), B = W companion [N][K] (K-major, per-tensor scale)
-extern "C" int gcbf_linear_fwd_t(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
-                                 const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream) {
+// Y[M,N] = act(alpha * X W^T + bias): A = X companion [M][K] (K-major), B = W companion [N][K] (K-major, per-tensor scale).
+// products: 3 (3xFP16) or 1 (fp16: the hi planes only; the companions keep their [hi|lo] format)
+extern "C" int gcbf_linear_fwd_tp(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
+                                  const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream, int products) {
   GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && (Y || Yh) && (!Y || ldy >= N), "gcbf_linear_fwd_t: bad arguments M=%d N=%d K=%d", M, N, K);
+  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_fwd_tp: products %d (3 or 1)", products);
   if (int rc = check_h16(X, "gcbf_linear_fwd_t X", M, K)) return rc;
   if (int rc = check_h16(W, "gcbf_linear_fwd_t W", N, K)) return rc;
   GCBF_REQUIRE(W->amax_row_stride == 0 && W->amax_col_stride == 0, "gcbf_linear_fwd_t: the weight companion must be per-tensor scaled");
@@ -826,15 +866,21 @@ extern "C" int gcbf_linear_fwd_t(const gcbf_h16* X, const gcbf_h16* W, const flo
     oh = th::OutH{reinterpret_cast<__half*>(Yh->buf), M, N, Yh->ld, reinterpret_cast<uint32_t*>(Yh->amax), Yh->amax_row_stride};
   }
   th::Operand A{reinterpret_cast<const __half*>(X->buf), M, K, X->ld, false}, B{reinterpret_cast<const __half*>(W->buf), N, K, W->ld, false};
-  return (N > 128) ? th::launch<256, false, false>(A, B, Y, ldy, M, N, K, 1, ep, Yh ? &oh : nullptr, st)
-                   : th::launch<128, false, false>(A, B, Y, ldy, M, N, K, 1, ep, nullptr, st);
+  return (N > 128) ? th::launch_p<256, false, false>(products, A, B, Y, ldy, M, N, K, 1, ep, Yh ? &oh : nullptr, st)
+                   : th::launch_p<128, false, false>(products, A, B, Y, ldy, M, N, K, 1, ep, nullptr, st);
+}
+
+extern "C" int gcbf_linear_fwd_t(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
+                                 const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream) {
+  return gcbf_linear_fwd_tp(X, W, bias, inv_sigma, act, Y, ldy, Yh, out_amax, M, N, K, stream, 3);
 }
 
 // dX[M,K] (+)= alpha * dZ W (* relu mask): A = dZ companion [M][N] (K-major: contraction over N), B = W companion [N][K] (MN-major)
-extern "C" int gcbf_linear_bwd_data_t(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
-                                      const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
-                                      void* out_amax, int M, int N, int K, void* stream) {
+extern "C" int gcbf_linear_bwd_data_tp(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
+                                       const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
+                                       void* out_amax, int M, int N, int K, void* stream, int products) {
   GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && (dX || dXh) && (!dX || lddx >= K), "gcbf_linear_bwd_data_t: bad arguments M=%d N=%d K=%d", M, N, K);
+  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_bwd_data_tp: products %d (3 or 1)", products);
   GCBF_REQUIRE(!relu_src || ld_relu >= K, "gcbf_linear_bwd_data_t: ld_relu");
   GCBF_REQUIRE(!(relu_src && relu_h) && !(accumulate && (dXh || colsum)), "gcbf_linear_bwd_data_t: conflicting options");
   if (int rc = check_h16(dZ, "gcbf_linear_bwd_data_t dZ", M, N)) return rc;
@@ -857,14 +903,21 @@ extern "C" int gcbf_linear_bwd_data_t(const gcbf_h16* dZ, const gcbf_h16* W, con
     oh = th::OutH{reinterpret_cast<__half*>(dXh->buf), M, K, dXh->ld, reinterpret_cast<uint32_t*>(dXh->amax), dXh->amax_row_stride};
   }
   th::Operand A{reinterpret_cast<const __half*>(dZ->buf), M, N, dZ->ld, false}, B{reinterpret_cast<const __half*>(W->buf), N, K, W->ld, true};
-  return (K > 128) ? th::launch<256, false, true>(A, B, dX, lddx, M, K, N, 1, ep, dXh ? &oh : nullptr, st)
-                   : th::launch<128, false, true>(A, B, dX, lddx, M, K, N, 1, ep, nullptr, st);
+  return (K > 128) ? th::launch_p<256, false, true>(products, A, B, dX, lddx, M, K, N, 1, ep, dXh ? &oh : nullptr, st)
+                   : th::launch_p<128, false, true>(products, A, B, dX, lddx, M, K, N, 1, ep, nullptr, st);
+}
+
+extern "C" int gcbf_linear_bwd_data_t(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
+                                      const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
+                                      void* out_amax, int M, int N, int K, void* stream) {
+  return gcbf_linear_bwd_data_tp(dZ, W, inv_sigma, relu_src, ld_relu, relu_h, dX, lddx, accumulate, dXh, colsum, out_amax, M, N, K, stream, 3);
 }
 
 // dW[N,K] (+)= alpha * dZ^T X: A = dZ companion [M][N] (MN-major), B = X companion [M][K] (MN-major); contraction over M
-extern "C" int gcbf_linear_bwd_weight_t(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
-                                        int M, int N, int K, void* stream) {
+extern "C" int gcbf_linear_bwd_weight_tp(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
+                                         int M, int N, int K, void* stream, int products) {
   GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && lddw >= K && dW, "gcbf_linear_bwd_weight_t: bad arguments M=%d N=%d K=%d", M, N, K);
+  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_bwd_weight_tp: products %d (3 or 1)", products);
   if (int rc = check_h16(dZ, "gcbf_linear_bwd_weight_t dZ", M, N)) return rc;
   if (int rc = check_h16(X, "gcbf_linear_bwd_weight_t X", M, K)) return rc;
   cudaStream_t st = as_stream(stream);
@@ -877,8 +930,13 @@ extern "C" int gcbf_linear_bwd_weight_t(const gcbf_h16* dZ, const gcbf_h16* X, c
   int splits = 1;
   if (tiles < kNumSMs) splits = max(1, min(ceil_div(M, 256), kNumSMs / tiles));
   th::Operand A{reinterpret_cast<const __half*>(dZ->buf), M, N, dZ->ld, true}, B{reinterpret_cast<const __half*>(X->buf), M, K, X->ld, true};
-  return (BN == 256) ? th::launch<256, true, true>(A, B, dW, lddw, N, K, M, splits, ep, nullptr, st)
-                     : th::launch<128, true, true>(A, B, dW, lddw, N, K, M, splits, ep, nullptr, st);
+  return (BN == 256) ? th::launch_p<256, true, true>(products, A, B, dW, lddw, N, K, M, splits, ep, nullptr, st)
+                     : th::launch_p<128, true, true>(products, A, B, dW, lddw, N, K, M, splits, ep, nullptr, st);
+}
+
+extern "C" int gcbf_linear_bwd_weight_t(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
+                                        int M, int N, int K, void* stream) {
+  return gcbf_linear_bwd_weight_tp(dZ, X, inv_sigma, dW, lddw, accumulate, M, N, K, stream, 3);
 }
 
 // ---- the per-tensor-scaled entry points of ABI v2: thin wrappers ------------------------------------------------------------------------

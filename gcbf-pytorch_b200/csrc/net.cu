@@ -171,7 +171,7 @@ static H16 alloc_tiled(Run& R, int rows, int cols) {
 // if need_f32_out.
 int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, int ldx, int M, const H16* x_h, const void* x_amax,
                 int next_width, const float* const* inv_sigma, const float* const* us, const float* const* vs, MlpCtx* ctx, float* out,
-                int ld_out, bool need_f32_out, H16* out_h, const float** y, int* ldy, const void** y_amax) {
+                int ld_out, bool need_f32_out, H16* out_h, const float** y, int* ldy, const void** y_amax, int products) {
   if (ctx) { memset(ctx, 0, sizeof(*ctx)); ctx->n = n; ctx->M = M; ctx->acts[0] = x; ctx->ld[0] = ldx; }
   const float* cur = x;
   int ldc = ldx;
@@ -201,7 +201,7 @@ int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, i
       if (!R.dry) {
         Timed t(R, 0, 2.0 * M * N * K, M, N, K);
         const gcbf_h16 X = h16_desc(cur_h), W = weight_desc(L), Y = h16_desc(yh);
-        CHAIN_CALL(gcbf_linear_fwd_t(&X, &W, L.b, inv_sigma[l], L.act, dst, ldd, emit ? &Y : nullptr, ya, M, N, K, R.st));
+        CHAIN_CALL(gcbf_linear_fwd_tp(&X, &W, L.b, inv_sigma[l], L.act, dst, ldd, emit ? &Y : nullptr, ya, M, N, K, R.st, products));
         R.launched(1);
       }
     } else if (sk_emit) {
@@ -254,7 +254,8 @@ int vec_add(Run& R, float* dst, const float* src, int64_t n) {
 // qualifies, dx is emitted as a companion only (*dx == nullptr, dx_h->buf != nullptr) and its column sums are added to dx_colsum.
 int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ctx, const float* dy, int ld_dy, const H16* dy_h,
                  bool dy_colsum_done, bool need_dx, float* dx_out, int ld_dx, bool dx_accumulate, const void* dy_amax, void* dx_amax,
-                 bool skip_wgrad, H16* dx_h, int dx_consumer_n, float* dx_colsum, const float** dx, int* ld_dx_res, bool* dx_amax_valid) {
+                 bool skip_wgrad, H16* dx_h, int dx_consumer_n, float* dx_colsum, const float** dx, int* ld_dx_res, bool* dx_amax_valid,
+                 int products) {
   const int M = ctx.M;
   const int last = n - 1;
   const float* dz = dy;
@@ -296,13 +297,13 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
           float* fx = (float*)R.ws.alloc(gcbf_sn_workspace_floats(N, K) * 4);
           if (!R.dry) {
             { Timed t(R, 2, 2.0 * M * N * K, M, N, K);
-              CHAIN_CALL(gcbf_linear_bwd_weight_t(&dZ, &X, isg, dW, K, 0, M, N, K, R.st)); }
+              CHAIN_CALL(gcbf_linear_bwd_weight_tp(&dZ, &X, isg, dW, K, 0, M, N, K, R.st, products)); }
             CHAIN_CALL(gcbf_sn_grad_fixup(dW, K, L.W, L.ldw, N, K, ctx.u[l], ctx.v[l], isg, fx, L.gW, L.ldgw, R.st));
             R.launched(3);
           }
         } else if (!R.dry) {
           Timed t(R, 2, 2.0 * M * N * K, M, N, K);
-          CHAIN_CALL(gcbf_linear_bwd_weight_t(&dZ, &X, isg, L.gW, L.ldgw, 1, M, N, K, R.st));
+          CHAIN_CALL(gcbf_linear_bwd_weight_tp(&dZ, &X, isg, L.gW, L.ldgw, 1, M, N, K, R.st, products));
           R.launched(1);
         }
       }
@@ -320,8 +321,8 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
         if (!R.dry) {
           Timed t(R, 1, 2.0 * M * N * K, M, N, K);
           const gcbf_h16 O = h16_desc(oh);
-          CHAIN_CALL(gcbf_linear_bwd_data_t(&dZ, &W, isg, mask_h ? nullptr : x_in, ldx, mask_h ? &maskh : nullptr, o, K, 0, emit ? &O : nullptr,
-                                            (emit && pw) ? P.gb : nullptr, na, M, N, K, R.st));
+          CHAIN_CALL(gcbf_linear_bwd_data_tp(&dZ, &W, isg, mask_h ? nullptr : x_in, ldx, mask_h ? &maskh : nullptr, o, K, 0, emit ? &O : nullptr,
+                                             (emit && pw) ? P.gb : nullptr, na, M, N, K, R.st, products));
           R.launched(1);
         }
         dz = o; lddz = K; dz_amax = na; dzh = oh; colsum_done = emit && pw;
@@ -334,8 +335,8 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
         if (!R.dry) {
           Timed t(R, 1, 2.0 * M * N * K, M, N, K);
           const gcbf_h16 O = h16_desc(oh);
-          CHAIN_CALL(gcbf_linear_bwd_data_t(&dZ, &W, isg, nullptr, 0, nullptr, o, ldo, dx_accumulate ? 1 : 0, emit ? &O : nullptr,
-                                            (emit && !skip_wgrad) ? dx_colsum : nullptr, emit ? nullptr : dx_amax, M, N, K, R.st));
+          CHAIN_CALL(gcbf_linear_bwd_data_tp(&dZ, &W, isg, nullptr, 0, nullptr, o, ldo, dx_accumulate ? 1 : 0, emit ? &O : nullptr,
+                                             (emit && !skip_wgrad) ? dx_colsum : nullptr, emit ? nullptr : dx_amax, M, N, K, R.st, products));
           R.launched(1);
         }
         dz = o; lddz = ldo;
@@ -417,12 +418,20 @@ int collect_layers(const gcbf_net_desc& net, const gcbf_linear_desc** all) {
   return n;
 }
 
+// fp16 products per k-slice of the net's tensor-core layers (gcbf_net_desc.tc_products: 0 = the 3xFP16 default).  Only the wgmma
+// launches see it: the dispatch rule and the fp32 kernels of the narrow layers are the same in both modes.
+static int tc_products(const gcbf_net_desc& net) { return net.tc_products == 1 ? 1 : 3; }
+
 int check_net(const gcbf_net_desc* net) {
   if (!net) { set_error("null net descriptor"); return GCBF_E_INVALID; }
   if (int rc = check_mlp(net->phi, net->n_phi, "phi")) return rc;
   if (int rc = check_mlp(net->gate, net->n_gate, "gate_nn")) return rc;
   if (int rc = check_mlp(net->gamma, net->n_gamma, "gamma")) return rc;
   if (net->n_head && check_mlp(net->head, net->n_head, "head")) return GCBF_E_INVALID;
+  if (net->tc_products != 0 && net->tc_products != 3 && net->tc_products != 1) {
+    set_error("net descriptor: tc_products %d (0 or 3: 3xFP16, 1: one fp16 product)", net->tc_products);
+    return GCBF_E_INVALID;
+  }
   const int kin = 2 * net->node_dim + net->edge_dim;
   if (net->phi[0].K != kin || net->phi[net->n_phi - 1].N != net->phi_dim || net->gate[0].K != net->phi_dim ||
       net->gate[net->n_gate - 1].N != 1 || net->gamma[0].K != net->phi_dim + net->node_dim ||
@@ -438,6 +447,7 @@ int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* e
                 int ld_out, NetCtx* ctx, const float* const* inv_sigma_in) {
   const int E = (int)E64;
   const int nd = net.node_dim, C = net.phi_dim, kin = 2 * nd + net.edge_dim;
+  const int tp = tc_products(net);
   const bool save = ctx != nullptr;
   if (ctx) { memset(ctx, 0, sizeof(*ctx)); ctx->E = E; ctx->Nn = Nn; ctx->R = rows; }
   float* ein = (float*)R.ws.alloc((size_t)E * kin * 4);
@@ -461,9 +471,9 @@ int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* e
   // phi's output is needed twice: as fp32 by the aggregation and (as a companion, when the gate's first layer is a tensor-core
   // layer) by gate_nn -- the last phi layer writes both
   if (int rc = mlp_forward(R, net.phi, net.n_phi, ein, kin, E, nullptr, nullptr, net.gate[0].N, isg, us, vs, save ? &ctx->phi : nullptr, nullptr, 0,
-                           true, &msg_h, &msg, &ldm, &msg_amax)) return rc;                      // gnn.py:30-32
+                           true, &msg_h, &msg, &ldm, &msg_amax, tp)) return rc;                      // gnn.py:30-32
   if (int rc = mlp_forward(R, net.gate, net.n_gate, msg, ldm, E, msg_h.buf ? &msg_h : nullptr, msg_amax, 0, isg + o_gate, us + o_gate, vs + o_gate,
-                           save ? &ctx->gate : nullptr, nullptr, 0, true, nullptr, &gate, &ldg, nullptr)) return rc;   // AttentionalAggregation.gate_nn
+                           save ? &ctx->gate : nullptr, nullptr, 0, true, nullptr, &gate, &ldg, nullptr, tp)) return rc;   // AttentionalAggregation.gate_nn
   float* gin_all = (float*)R.ws.alloc((size_t)Nn * (C + nd) * 4);
   float* att = (float*)R.ws.alloc((size_t)E * 4);
   if (!R.dry) {
@@ -482,7 +492,7 @@ int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* e
   // gamma's output feeds the head directly when nothing is concatenated (CBF): then only its companion is written
   if (int rc = mlp_forward(R, net.gamma, net.n_gamma, gin, C + nd, rows, nullptr, nullptr, chain_head ? net.head[0].N : 0, isg + o_gamma,
                            us + o_gamma, vs + o_gamma, save ? &ctx->gamma : nullptr, has_head ? nullptr : out, ld_out, !chain_head,
-                           chain_head ? &feat_h : nullptr, &feat, &ldf, &feat_amax)) return rc;   // gnn.py:34-36
+                           chain_head ? &feat_h : nullptr, &feat, &ldf, &feat_amax, tp)) return rc;   // gnn.py:34-36
   if (has_head) {
     const int F = net.gamma[net.n_gamma - 1].N;
     const float* hin = feat;
@@ -499,7 +509,7 @@ int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* e
     const float* y; int ldy;
     if (int rc = mlp_forward(R, net.head, net.n_head, hin, ldh, rows, (chain_head && feat_h.buf) ? &feat_h : nullptr,
                              chain_head ? feat_amax : nullptr, 0, isg + o_head, us + o_head, vs + o_head, save ? &ctx->head : nullptr, out,
-                             ld_out, true, nullptr, &y, &ldy, nullptr)) return rc;
+                             ld_out, true, nullptr, &y, &ldy, nullptr, tp)) return rc;
   }
   if (ctx) { ctx->msg = msg; ctx->att = att; }
   return 0;
@@ -509,6 +519,7 @@ int net_backward(Run& R, const gcbf_net_desc& net, const NetCtx& ctx, const int3
                  const float* d_out, int ld_dout, float* d_edge_attr, bool skip_wgrad, cudaEvent_t gamma_done) {
   const int E = ctx.E, Nn = ctx.Nn, rows = ctx.R;
   const int nd = net.node_dim, C = net.phi_dim;
+  const int tp = tc_products(net);
   const float* d_feat = d_out;
   int ld_dfeat = ld_dout;
   const void* d_feat_amax = nullptr;
@@ -522,13 +533,13 @@ int net_backward(Run& R, const gcbf_net_desc& net, const NetCtx& ctx, const int3
     // sides are tensor-core layers (with gamma's last bias gradient = its column sums)
     const bool direct = net.head_extra_dim == 0;
     if (int rc = mlp_backward(R, net.head, net.n_head, ctx.head, d_out, ld_dout, nullptr, false, true, nullptr, 0, false, nullptr, slot, skip_wgrad,
-                              direct ? &d_feat_h : nullptr, GL.K, g_colsum ? GL.gb : nullptr, &d_hin, &ld_dhin, &valid)) return rc;
+                              direct ? &d_feat_h : nullptr, GL.K, g_colsum ? GL.gb : nullptr, &d_hin, &ld_dhin, &valid, tp)) return rc;
     d_feat = d_hin; ld_dfeat = ld_dhin;         // the first F columns of d_hin (strided view when u_ref was concatenated)
     if (valid) d_feat_amax = slot;              // max over all of d_hin >= max over the d_feat columns: a valid (pow2) scale bound
   }
   const float* d_gin; int ld_dgin;
   if (int rc = mlp_backward(R, net.gamma, net.n_gamma, ctx.gamma, d_feat, ld_dfeat, d_feat_h.buf ? &d_feat_h : nullptr, g_colsum, true, nullptr, 0,
-                            false, d_feat_amax, nullptr, skip_wgrad, nullptr, 0, nullptr, &d_gin, &ld_dgin, nullptr)) return rc;
+                            false, d_feat_amax, nullptr, skip_wgrad, nullptr, 0, nullptr, &d_gin, &ld_dgin, nullptr, tp)) return rc;
   if (gamma_done && !R.dry) CHAIN_CUDA(cudaEventRecord(gamma_done, R.st));     // head + gamma gradients of this pass are enqueued
   const float* d_gin_all = d_gin;
   int ld_dga = ld_dgin;
@@ -552,10 +563,10 @@ int net_backward(Run& R, const gcbf_net_desc& net, const NetCtx& ctx, const int3
   void* slot = R.amax_slot();
   bool valid = false;
   if (int rc = mlp_backward(R, net.gate, net.n_gate, ctx.gate, d_gate, 1, nullptr, false, true, d_msg, C, true, nullptr, slot, skip_wgrad, nullptr, 0,
-                            nullptr, nullptr, nullptr, &valid)) return rc;
+                            nullptr, nullptr, nullptr, &valid, tp)) return rc;
   const float* d_ein; int ld_dein;
   if (int rc = mlp_backward(R, net.phi, net.n_phi, ctx.phi, d_msg, C, nullptr, false, d_edge_attr != nullptr, nullptr, 0, false,
-                            valid ? slot : nullptr, nullptr, skip_wgrad, nullptr, 0, nullptr, &d_ein, &ld_dein, nullptr)) return rc;
+                            valid ? slot : nullptr, nullptr, skip_wgrad, nullptr, 0, nullptr, &d_ein, &ld_dein, nullptr, tp)) return rc;
   if (d_edge_attr && !R.dry && E > 0) {
     CHAIN_CALL(gcbf_copy2d(d_ein + 2 * nd, ld_dein, d_edge_attr, net.edge_dim, E, net.edge_dim, R.st));
     R.launched(1);
@@ -686,7 +697,7 @@ static int mlp_fwd_run(Run& R, const gcbf_linear_desc* layers, int n, int refres
   if (int rc = sn_power_iter(R, all, n, ctx != nullptr, isg, us, vs)) return rc;
   if (refresh) { if (int rc = refresh_weight_companions(R, all, n)) return rc; }
   const float* y; int ldy;
-  return mlp_forward(R, layers, n, x, ldx, rows, nullptr, nullptr, 0, isg, us, vs, ctx, out, ld_out, true, nullptr, &y, &ldy, nullptr);
+  return mlp_forward(R, layers, n, x, ldx, rows, nullptr, nullptr, 0, isg, us, vs, ctx, out, ld_out, true, nullptr, &y, &ldy, nullptr, 3);
 }
 
 extern "C" size_t gcbf_mlp_forward_workspace_bytes(const gcbf_linear_desc* layers, int n_layers, int rows, int save_ctx) {
@@ -706,7 +717,7 @@ extern "C" size_t gcbf_mlp_backward_workspace_bytes(const gcbf_linear_desc* laye
   if (mlp_fwd_run(F, layers, n_layers, 0, &dummy, layers[0].K, rows, &dummy, layers[n_layers - 1].N, &ctx)) return 0;
   Run B(nullptr, 0, nullptr, true);
   if (mlp_backward(B, layers, n_layers, ctx, &g_dummy_f, layers[n_layers - 1].N, nullptr, false, true, nullptr, 0, false, nullptr, nullptr, false, nullptr, 0, nullptr,
-                   nullptr, nullptr, nullptr)) return 0;
+                   nullptr, nullptr, nullptr, 3)) return 0;
   return B.ws.off + 1024;
 }
 
@@ -729,6 +740,6 @@ extern "C" int gcbf_mlp_backward(const gcbf_linear_desc* layers, int n_layers, c
   Run R(workspace, workspace_bytes, as_stream(stream), false);
   const MlpCtx& c = *reinterpret_cast<const MlpCtx*>(ctx);
   int rc = mlp_backward(R, layers, n_layers, c, d_out, ld_dout, nullptr, false, d_x != nullptr, d_x, layers[0].K, false, nullptr, nullptr,
-                        skip_wgrad != 0, nullptr, 0, nullptr, nullptr, nullptr, nullptr);
+                        skip_wgrad != 0, nullptr, 0, nullptr, nullptr, nullptr, nullptr, 3);
   return R.finish(rc, "gcbf_mlp_backward");
 }

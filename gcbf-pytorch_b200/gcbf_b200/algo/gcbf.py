@@ -12,6 +12,7 @@ What changes relative to the reference's `update` body (results identical, see t
 """
 import ctypes
 import os
+import weakref
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -106,6 +107,7 @@ class GCBF(Algorithm):
             'alpha': 1.0, 'eps': 0.02, 'inner_iter': 10, 'loss_action_coef': 0.001, 'loss_unsafe_coef': 1.,
             'loss_safe_coef': 1., 'loss_h_dot_coef': 0.1}
         self.process_group = None   # set to a torch.distributed group for data-parallel training
+        self._matmul_mode()         # validates params['matmul'] and puts the mode on the two modules
 
     def _build_networks(self, num_agents: int, node_dim: int, edge_dim: int, action_dim: int, device):
         # models: same construction order as the reference (gcbf.py:87-100) => same seeded initialisation
@@ -116,10 +118,12 @@ class GCBF(Algorithm):
     # ---- rollout-time API ---------------------------------------------------------------------------
     @torch.no_grad()
     def act(self, data) -> Tensor:
+        self._matmul_mode()
         return self.actor(data)
 
     @torch.no_grad()
     def step(self, data, prob: float) -> Tensor:
+        self._matmul_mode()
         action = self.actor(data)
         if np.random.rand() < prob:
             action = torch.zeros_like(action)
@@ -171,7 +175,9 @@ class GCBF(Algorithm):
         workspace: valid until the next train_step of this object).
         params['h_dot'] selects the CBF-condition loss: 'finite_difference' (the default, the reference's) or 'analytic'
         (_train_step_analytic)."""
+        self._matmul_mode()
         if self._h_dot_mode() == 'analytic':
+            self._refuse_fp16("params['h_dot'] = 'analytic' training")
             return self._train_step_analytic(graphs, apply_optim, compute_acc_h_dot)
         if ops.NATIVE:
             return self._train_step_native(graphs, apply_optim, compute_acc_h_dot)
@@ -183,6 +189,42 @@ class GCBF(Algorithm):
             ARENA.end()
 
     H_DOT_MODES = ('finite_difference', 'analytic')
+    MATMUL_MODES = ('fp32', 'fp16')
+
+    def _matmul_mode(self) -> str:
+        """params['matmul']: 'fp32' (default; 3xFP16 tensor-core products, fp32-grade) or 'fp16' (one fp16 product per k-slice in
+        the 2048-wide layers: faster, with the accuracy contract of DESIGN section 5).  The two modules read the key at every pass
+        (their layers hold a weak reference to this object), so self.cbf(data) / self.actor(data) -- rollouts, VectorRollout, the
+        Trainer -- run in the mode the key has at that moment.  Only the library-sequenced passes have the fp16 kernels: with
+        GCBF_NATIVE=0 'fp16' is refused."""
+        mode = self.params.get('matmul', 'fp32')
+        if mode not in self.MATMUL_MODES:
+            raise ValueError(f"params['matmul'] must be one of {self.MATMUL_MODES}, got {mode!r}")
+        if mode == 'fp16' and not ops.NATIVE:
+            raise ValueError("params['matmul'] = 'fp16' needs the library-sequenced passes (GCBF_NATIVE=1)")
+        for m in (self.cbf, self.actor):
+            layer = m.feat_transformer.module_0
+            if layer._matmul_owner is None or layer._matmul_owner() is not self:
+                layer._matmul_owner = weakref.ref(self)
+        return mode
+
+    def _matmul_products(self) -> int:
+        return ops.MATMUL_PRODUCTS[self._matmul_mode()]
+
+    def set_matmul(self, mode: str):
+        """Switch the tensor-core precision ('fp32' or 'fp16') of every later pass of both nets."""
+        old = self.params.get('matmul', 'fp32')
+        self.params['matmul'] = mode
+        try:
+            self._matmul_mode()
+        except ValueError:
+            self.params['matmul'] = old
+            raise
+        return self
+
+    def _refuse_fp16(self, what: str):
+        if self._matmul_mode() == 'fp16':
+            raise ValueError(f"{what} is sequenced in Python on the 3xFP16 kernels and does not run in params['matmul'] = 'fp16'")
 
     def _h_dot_mode(self) -> str:
         mode = self.params.get('h_dot', 'finite_difference')
@@ -336,7 +378,7 @@ class GCBF(Algorithm):
         from .. import native
         env, hp = self._env, self.params
         bucket = self._ensure_bucket()
-        key = (id(env), id(env._goal), env._goal.data_ptr() if env._goal is not None else 0, bucket.flat.data_ptr())
+        key = (id(env), id(env._goal), env._goal.data_ptr() if env._goal is not None else 0, bucket.flat.data_ptr(), self._matmul_mode())
         cached = getattr(self, '_native_desc', None)
         if cached is not None and cached[0] == key:
             return cached[1]
@@ -542,6 +584,7 @@ class GCBF(Algorithm):
         actions through forward_graph -> CBF (same kernels as training: K2, K3, K4, K5 forward and input-gradient),
         plus the reference's gradient noise `rand * lr * randn * grad`.  The per-agent optimisers are kept as one
         vectorised state (m, v, step count per agent); the O(num_agents) arithmetic around the kernels is host glue."""
+        self._matmul_mode()
         if ops.NATIVE and data.states.is_cuda:
             return self._apply_native(data, rand, max_iter, None, batched=False)
         return self._apply_python(data, rand, max_iter, None)
@@ -553,6 +596,7 @@ class GCBF(Algorithm):
         graph did go to `self.last_apply_batch_rounds` (host int tensor [B]).  noise: the standard normals of the gradient noise
         [(max_iter + 1), B * n, action_dim] (default: drawn here); round k of graph g reads its rows of slice k, so concatenated
         per-graph draws reproduce per-graph calls."""
+        self._matmul_mode()
         if ops.NATIVE and batch.states.is_cuda:
             return self._apply_native(batch, rand, max_iter, noise, batched=True)
         return self._apply_python(batch, rand, max_iter, noise)
@@ -666,6 +710,7 @@ class GCBF(Algorithm):
         derivative the finite difference (h(x + dt f) - h(x)) / dt of gcbf.py:193-207 approximates, edges held fixed.  action: the
         policy's correction (default: the actor's).  The CBF condition of the paper is h_dot + alpha h >= 0."""
         from .. import jvp
+        self._refuse_fp16('h_dot_analytic')
         if action is None:
             action = self.act(data)
         return jvp.cbf_value_and_h_dot(self.cbf, self._env, data, action, freeze)
@@ -701,6 +746,7 @@ class GCBF(Algorithm):
         call's largest chunk: at most max_probes probes with at most nodes_per_graph - 1 edges each, and at most max_edges edges."""
         import ctypes
         from .. import native
+        self._matmul_mode()
         d, keep, xs, ys, B, A, T = self._field_desc(data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges)
         layers = keep[-1]
         dev = data.states.device
@@ -752,6 +798,7 @@ class GCBF(Algorithm):
         of the CBF by ONE power iteration each and uses that 1/sigma in every chunk of at most max_probes probes / max_edges two-hop
         edges; one host sync per call (the per-probe counts).  The chunk count and the two-hop edges go to self.last_field_chunks /
         self.last_field_edges."""
+        self._refuse_fp16('cbf_condition_field')
         d, keep, xs, ys, B, A, T, plan = self._condition_plan(data, agents, x_dim, y_dim, n_mesh, lims, relink, max_probes, max_edges)
         from .. import jvp
         env = self._env

@@ -53,6 +53,14 @@ class MACBF(GCBF):
         self.params = params if params is not None else {
             'alpha': 1.0, 'eps': 0.02, 'inner_iter': 10, 'loss_action_coef': 0.001, 'loss_unsafe_coef': 1., 'loss_safe_coef': 1.,
             'loss_h_dot_coef': 0.1}
+        self._matmul_mode()
+
+    def _matmul_mode(self) -> str:
+        """MACBF's MLPs run on the bare-MLP entry points, which have the 3xFP16 kernels only."""
+        mode = self.params.get('matmul', 'fp32')
+        if mode != 'fp32':
+            raise ValueError(f"MACBF supports params['matmul'] = 'fp32' only, got {mode!r}")
+        return mode
 
     def _build_networks(self, num_agents: int, node_dim: int, edge_dim: int, action_dim: int, device):
         if self._reference_rng:

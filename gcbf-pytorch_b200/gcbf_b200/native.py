@@ -30,7 +30,7 @@ class NetDesc(ctypes.Structure):
     _fields_ = [('phi', LinearDesc * MAX_LAYERS), ('gate', LinearDesc * MAX_LAYERS), ('gamma', LinearDesc * MAX_LAYERS),
                 ('head', LinearDesc * MAX_LAYERS), ('n_phi', c_int32), ('n_gate', c_int32), ('n_gamma', c_int32), ('n_head', c_int32),
                 ('node_dim', c_int32), ('edge_dim', c_int32), ('phi_dim', c_int32), ('head_extra_dim', c_int32),
-                ('refresh_weights', c_int32), ('pad_', c_int32)]
+                ('refresh_weights', c_int32), ('tc_products', c_int32)]
 
 
 class NetCtx(ctypes.Structure):
@@ -117,8 +117,13 @@ SIGS = {
     'gcbf_linear_bwd_data_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
                                        c_int, c_int, c_int, P]),
     'gcbf_linear_bwd_weight_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, c_int, c_int, c_int, c_int, P]),
+    'gcbf_linear_fwd_tp': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P, c_int]),
+    'gcbf_linear_bwd_data_tp': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
+                                        c_int, c_int, c_int, P, c_int]),
+    'gcbf_linear_bwd_weight_tp': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, c_int, c_int, c_int, c_int, P, c_int]),
     'gcbf_linear_fwd_emit': (c_int, [P, c_int, P, c_int, P, P, c_int, POINTER(H16Desc), c_int, c_int, c_int, P]),
     'gcbf_launch_count': (c_longlong, [c_int]),
+    'gcbf_tc_launch_count': (c_longlong, [c_int, c_int]),
     'gcbf_timing_enable': (c_int, [c_int]),
     'gcbf_timing_collect': (c_int, [POINTER(TimeRec), c_int, POINTER(c_int)]),
     'gcbf_set_gemm_impl': (c_int, [c_int]),
@@ -211,6 +216,7 @@ def make_net_desc(spec, head_extra_dim: int, grads, force_h: bool = False, grad_
         setattr(nd, 'n_' + name, len(layers))
     nd.node_dim, nd.edge_dim, nd.phi_dim = spec.node_dim, spec.edge_dim, spec.phi_dim
     nd.head_extra_dim = head_extra_dim if spec.head else 0
+    nd.tc_products = spec.tc_products
     return nd
 
 
@@ -250,3 +256,8 @@ def view(ws: torch.Tensor, ptr: int, shape, dtype) -> torch.Tensor:
 
 def launch_count(reset: bool = False) -> int:
     return int(fn('gcbf_launch_count')(1 if reset else 0))
+
+
+def tc_launch_count(products: int, reset: bool = False) -> int:
+    """wgmma launches so far with `products` (3 or 1) fp16 products per k-slice."""
+    return int(fn('gcbf_tc_launch_count')(products, 1 if reset else 0))

@@ -70,6 +70,8 @@ def prime_rowptr(edge_index: Tensor, num_nodes: int) -> Tensor:
 
 class _GNNLayerBase(nn.Module):
     limit_lip = False
+    tc_products = 3         # fp16 products per k-slice of the tensor-core layers: 3 (3xFP16, default) or 1 (fp16) -- for a layer no algorithm owns
+    _matmul_owner = None    # weakref to the GCBF whose params['matmul'] decides the mode, read at every pass
 
     def __init__(self, node_dim: int, edge_dim: int, output_dim: int, phi_dim: int):
         super().__init__()
@@ -82,10 +84,16 @@ class _GNNLayerBase(nn.Module):
                          limit_lip=self.limit_lip)
         self._dims = (node_dim, edge_dim, phi_dim)
 
+    def products(self) -> int:
+        """fp16 products per k-slice of this layer's tensor-core launches: the owning GCBF's params['matmul'] as it is now (so a
+        changed key reaches every later pass, rollouts included), else `tc_products`."""
+        owner = self._matmul_owner() if self._matmul_owner is not None else None
+        return owner._matmul_products() if owner is not None else self.tc_products
+
     def net_spec(self, head: Optional[MLP] = None) -> ops.NetSpec:
         nd, ed, pd = self._dims
         return ops.NetSpec(self.phi.specs(), self.aggr_module.gate_nn.specs(), self.gamma.specs(),
-                           head.specs() if head is not None else None, nd, ed, pd)
+                           head.specs() if head is not None else None, nd, ed, pd, self.products())
 
     def run(self, x: Tensor, edge_attr: Tensor, edge_index: Tensor, row_index: Optional[Tensor] = None,
             head: Optional[MLP] = None, head_extra: Optional[Tensor] = None) -> Tensor:
@@ -107,6 +115,8 @@ class _GNNLayerBase(nn.Module):
     def attention(self, data) -> Tensor:
         """Attention weights [E, 1] (reference gnn.py:44-53); inference helper, no autograd."""
         spec = self.net_spec()
+        if spec.tc_products != 3:
+            raise ValueError("attention() is sequenced in Python on the 3xFP16 kernels and does not run in params['matmul'] = 'fp16'")
         with torch.no_grad():
             E = data.edge_index.shape[1]
             ein = torch.empty(E, 2 * spec.node_dim + spec.edge_dim, device=data.x.device)

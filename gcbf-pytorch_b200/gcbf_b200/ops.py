@@ -897,6 +897,11 @@ class MLPFunction(torch.autograd.Function):
 # ----------------------------------------------------------------------------------------------------
 # GNN layer (+ optional fused head)
 # ----------------------------------------------------------------------------------------------------
+# GCBF.params['matmul'] -> fp16 products per k-slice of the wgmma GEMM (gcbf_net_desc.tc_products): 'fp32' = 3xFP16 (fp32-grade, the
+# default), 'fp16' = one fp16 product (about 2^-10 relative per product, up to three times the tensor rate)
+MATMUL_PRODUCTS = {'fp32': 3, 'fp16': 1}
+
+
 @dataclass
 class NetSpec:
     phi: List[LinearSpec]
@@ -906,6 +911,7 @@ class NetSpec:
     node_dim: int = 4
     edge_dim: int = 4
     phi_dim: int = 256
+    tc_products: int = 3        # fp16 products per k-slice of the tensor-core layers (MATMUL_PRODUCTS); library-sequenced passes only
 
     def all_layers(self):
         return self.phi + self.gate + self.gamma + (self.head or [])
@@ -915,6 +921,9 @@ def net_forward(spec: NetSpec, x, edge_attr, edge_index, rowptr, row_index, head
     """phi -> attention aggregation -> gamma (on `row_index` rows only when given) -> head.
     Returns (out, ctx-tuple).  sigma: (inv_sigmas, uvs) of an earlier sn_power_iter_batched(spec.all_layers()) to use instead of a
     new power iteration (passes that share one spectral-norm step, e.g. the chunks of one field call)."""
+    if spec.tc_products != 3:
+        raise ValueError("the fp16 matmul mode runs in the library-sequenced passes only (GCBF_NATIVE=1); this pass is "
+                         "sequenced in Python at 3xFP16")
     dev = x.device
     E = edge_index.shape[1]
     Nn = x.shape[0]

@@ -179,6 +179,18 @@ int gcbf_linear_bwd_data_t(const gcbf_h16* dZ, const gcbf_h16* W, const float* i
                            void* out_amax, int M, int N, int K, void* stream);
 int gcbf_linear_bwd_weight_t(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
                              int M, int N, int K, void* stream);
+/* The same three products with the number of fp16 products per k-slice: 3 = hi*hi + lo*hi + hi*lo (what the _t functions run),
+ * 1 = hi*hi only (fp16 operands, one wgmma per k-slice; the lo planes are not read).  Any other value is an argument error. */
+int gcbf_linear_fwd_tp(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
+                       const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream, int products);
+int gcbf_linear_bwd_data_tp(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
+                            const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
+                            void* out_amax, int M, int N, int K, void* stream, int products);
+int gcbf_linear_bwd_weight_tp(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
+                              int M, int N, int K, void* stream, int products);
+/* wgmma launches issued so far with `products` (3 or 1) fp16 products per k-slice (reset != 0: and set the count to 0): which kernels
+ * a pass actually ran, e.g. that every tensor-core layer of a net in fp16 mode took the one-product kernels.  -1 for other values. */
+long long gcbf_tc_launch_count(int products, int reset);
 /* the skinny-K fp32 forward (in-features <= 16: the first phi layer, gnn.py:31) writing ONLY the tile-scaled companion of its output
  * (each 128 x 256 tile is computed twice: once for its exact maximum, once to convert and store) */
 int gcbf_linear_fwd_emit(const float* X, int ldx, const float* W, int ldw, const float* bias, const float* inv_sigma, int act,
@@ -344,7 +356,7 @@ typedef struct gcbf_net_desc {
   int32_t node_dim, edge_dim, phi_dim;
   int32_t head_extra_dim;                   /* columns concatenated to gamma's output before the head (u_ref: action_dim), or 0 */
   int32_t refresh_weights;                  /* != 0: the weights changed since the companions were made -> re-split them first */
-  int32_t pad_;
+  int32_t tc_products;                      /* 0 or 3: 3xFP16 (default), 1: one fp16 product -- the net's tensor-core layers only */
 } gcbf_net_desc;
 
 /* what a forward saves for its backward: pointers into the forward's workspace (which must stay alive and untouched) */
