@@ -168,6 +168,18 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
     setmaxnreg_dec<40>();
     // ===== TMA producer =====
     if (threadIdx.x == 0) {
+      // data-grad: once the first ring of loads is out, the tile's ReLU mask rows are requested into L2, so the epilogue does not
+      // wait on HBM for them.  Whole 16-byte pieces inside the tile's columns only (a ragged tail is left to the epilogue's loads).
+      bool mask_pending = MODE == EPI_DGRAD && (ep.relu_hi || ep.relu_src);
+      auto prefetch_mask = [&]() {
+        const int cols = min(BN, No - n0t), rows = min(BM, Mo - m0);
+        const bool vec = !ep.relu_src || ((ep.ld_relu & 3) == 0 && (reinterpret_cast<uintptr_t>(ep.relu_src) & 15) == 0);
+        const uint32_t bytes = (uint32_t)(cols * (ep.relu_src ? 4 : 2)) & ~15u;
+        if (vec && bytes)
+          for (int r = 0; r < rows; ++r)
+            bulk_prefetch_l2(ep.relu_src ? static_cast<const void*>(ep.relu_src + (size_t)(m0 + r) * ep.ld_relu + n0t)
+                                         : static_cast<const void*>(ep.relu_hi + (size_t)(m0 + r) * ep.ld_relu_h + n0t), bytes);
+      };
       int stage = 0;
       uint32_t phase = 0;
       for (int sub = 0; sub < NSUB; ++sub) {
@@ -180,6 +192,7 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
           load_tile<B_MN>(st + B_OFF, &map_b_hi, &full[stage], n0t + sub * SUB_N, kb * BK, SUB_N);
           if (P == 3) load_tile<B_MN>(st + B_OFF + B_BYTES, &map_b_lo, &full[stage], n0t + sub * SUB_N, kb * BK, SUB_N);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (mask_pending && (stage == 0 || kb + 1 == kb1)) { prefetch_mask(); mask_pending = false; }
         }
       }
     }
@@ -308,9 +321,68 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
 #pragma unroll
         for (int u = 0; u < 4; ++u) bias4[u] = (col + u < No) ? __ldg(ep.bias + col + u) * inv_alpha : 0.f;
       }
+      // ---- ReLU mask of the data-grad (mask = src > 0 or hi > 0): all of this thread's mask entries are loaded before pass 1
+      // stores into the parked tile, so the global loads are in flight together instead of one row at a time behind those stores.
+      // Bit 4 i + u of mbits: row tid / CG4 + i ROWS_PER_ITER, column col + u.
+      constexpr int RPT = BM / ROWS_PER_ITER;      // rows per thread
+      const bool has_mask = MODE == EPI_DGRAD && (ep.relu_src || ep.relu_hi);
+      uint32_t mbits[RPT / 8];
+#pragma unroll
+      for (int w = 0; w < RPT / 8; ++w) mbits[w] = 0u;
+      if (has_mask && col < No) {
+        const int nv = min(4, No - col);
+        const bool vec = nv == 4 && (!ep.relu_src || ((ep.ld_relu & 3) == 0 && (reinterpret_cast<uintptr_t>(ep.relu_src) & 15) == 0));
+        uint4 raw[RPT];                            // four fp32 words, or four halves in .x / .y
+#pragma unroll
+        for (int i = 0; i < RPT; ++i) {
+          const int row = m0 + tid / CG4 + i * ROWS_PER_ITER;
+          raw[i] = make_uint4(0u, 0u, 0u, 0u);
+          if (row >= Mo) continue;
+          if (!ep.relu_src) {
+            const __half* q = ep.relu_hi + (size_t)row * ep.ld_relu_h + col;
+            if (vec) {                               // 8-byte aligned: the pitch is a multiple of 8 halves, col of 4
+              const uint2 h = __ldg(reinterpret_cast<const uint2*>(q));
+              raw[i].x = h.x; raw[i].y = h.y;
+            } else {
+              const unsigned short* qs = reinterpret_cast<const unsigned short*>(q);
+              raw[i].x = __ldg(qs);
+              if (nv > 1) raw[i].x |= (uint32_t)__ldg(qs + 1) << 16;
+              if (nv > 2) raw[i].y = __ldg(qs + 2);
+            }
+          } else {
+            const float* q = ep.relu_src + (size_t)row * ep.ld_relu + col;
+            if (vec) {
+              const float4 f = __ldg(reinterpret_cast<const float4*>(q));
+              raw[i] = make_uint4(__float_as_uint(f.x), __float_as_uint(f.y), __float_as_uint(f.z), __float_as_uint(f.w));
+            } else {
+              raw[i].x = __float_as_uint(__ldg(q));
+              if (nv > 1) raw[i].y = __float_as_uint(__ldg(q + 1));
+              if (nv > 2) raw[i].z = __float_as_uint(__ldg(q + 2));
+              if (nv > 3) raw[i].w = __float_as_uint(__ldg(q + 3));     // an unaligned source
+            }
+          }
+        }
+#pragma unroll
+        for (int i = 0; i < RPT; ++i) {
+          float x[4];
+          if (!ep.relu_src) {
+            const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&raw[i].x));
+            const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&raw[i].y));
+            x[0] = a.x; x[1] = a.y; x[2] = b.x; x[3] = b.y;
+          } else {
+            x[0] = __uint_as_float(raw[i].x); x[1] = __uint_as_float(raw[i].y);
+            x[2] = __uint_as_float(raw[i].z); x[3] = __uint_as_float(raw[i].w);
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u)
+            if (x[u] > 0.f) mbits[i / 8] |= 1u << (4 * (i % 8) + u);
+        }
+      }
       // ---- pass 1: finish the values in place: bias, alpha, activation / ReLU mask; out-of-range entries become exact zeros
       float tmax = 0.f;
-      for (int r = tid / CG4; r < BM; r += ROWS_PER_ITER) {
+#pragma unroll
+      for (int i = 0; i < RPT; ++i) {
+        const int r = tid / CG4 + i * ROWS_PER_ITER;
         const int row = m0 + r;
         float4* p = reinterpret_cast<float4*>(pk + r * PARK_PITCH);
         float v[4];
@@ -324,10 +396,7 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
             else if (ep.act == GCBF_ACT_TANH) y = tanhf(y);
           }
           const bool ok = row < Mo && col + u < No;
-          if (MODE == EPI_DGRAD && ok) {
-            if (ep.relu_src) y = (__ldg(ep.relu_src + (size_t)row * ep.ld_relu + col + u) > 0.f) ? y : 0.f;
-            else if (ep.relu_hi) y = (__half2float(ep.relu_hi[(size_t)row * ep.ld_relu_h + col + u]) > 0.f) ? y : 0.f;
-          }
+          if (has_mask && ok) y = ((mbits[i / 8] >> (4 * (i % 8) + u)) & 1u) ? y : 0.f;
           v[u] = ok ? y : 0.f;
           tmax = fmaxf(tmax, fabsf(v[u]));
         }
@@ -388,7 +457,9 @@ gemm_h_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constan
         }
       }
       if (ep.amax_out && !ep.accumulate) out_max = fmaxf(out_max, tmax);
-      if (MODE == EPI_DGRAD && ep.colsum) epi_sync();   // pass 1 of every thread (masking, out-of-range zeros) is in the parked tile
+      // the column sums read what pass 1 of every thread (masking, out-of-range zeros) wrote; with an emitted companion the tile-maximum
+      // barrier has already waited for it
+      if (MODE == EPI_DGRAD && ep.colsum && !ep.out_h) epi_sync();
       if (MODE == EPI_DGRAD && ep.colsum && tid < BN) {
         // column sums over the tile's rows (the bias gradient of the layer below = colsum of dZ); masked / out-of-range entries are 0
         const float* pc = (tid < SUB_N ? park0 : park1) + (tid & (SUB_N - 1));

@@ -47,6 +47,10 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
+// bring `bytes` (a multiple of 16) of global memory from a 16-byte aligned address into L2, without waiting for it
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gptr, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
+}
 
 // ---- warpgroup MMA ---------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
