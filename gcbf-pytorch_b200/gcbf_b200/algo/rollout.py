@@ -30,17 +30,22 @@ from ..data import Data
 
 class VectorRollout:
     def __init__(self, env, algo, num_envs: int, reset_check_every: int = 16, states: Optional[torch.Tensor] = None,
-                 goals: Optional[torch.Tensor] = None, reset_seed: Optional[int] = None):
+                 goals: Optional[torch.Tensor] = None, reset_seed: Optional[int] = None, first_env: int = 0):
         """states [num_envs * N, s] / goals [num_envs * n, goal_dim]: explicit initial conditions (e.g. synthetic BASELINE states:
         the reference's rejection sampler cannot place >~ 290 agents, SURVEY section 0); default: env.reset() per env.
 
         reset_seed: None keeps the host resets above.  An integer switches to device resets: the initial states are episode 0 of every
         env drawn by `gcbf_env_reset_batch` with this seed, and every done env is re-sampled on the device right after the step that
-        finished it (env e's episode k depends only on (reset_seed, e, k)).  In that mode the per-env step counters `t_dev` and
-        episode counters `episode` are device tensors and the host array `self.t` is NOT authoritative (it counts steps since
+        finished it (env e's episode k depends only on (reset_seed, first_env + e, k)).  In that mode the per-env step counters `t_dev`
+        and episode counters `episode` are device tensors and the host array `self.t` is NOT authoritative (it counts steps since
         construction); a reset that cannot place its points raises RuntimeError at the next step's edge-count sync (or
-        `check_resets()`)."""
+        `check_resets()`).
+
+        first_env: global id of local env 0 under device resets.  A rollout of num_envs = B with first_env = r B steps exactly envs
+        r B .. r B + B - 1 of one rollout over more envs with the same reset_seed (data-parallel training gives every rank its own
+        block of global envs this way)."""
         self.env, self.algo, self.B = env, algo, int(num_envs)
+        self.first_env = int(first_env)
         self.n, self.N = env.num_agents, env.nodes_per_graph
         self.dev = env.device
         self.reset_check_every = reset_check_every
@@ -80,7 +85,8 @@ class VectorRollout:
     def _device_reset(self, reach: Optional[torch.Tensor]):
         """One gcbf_env_reset_batch launch over the batch and an asynchronous copy of the failure flags (read by check_resets)."""
         from ..env.device_reset import reset_batch
-        reset_batch(self.env, self.states, self.goals, self.t_dev, self.episode, self._failed, self.reset_seed, reach=reach)
+        reset_batch(self.env, self.states, self.goals, self.t_dev, self.episode, self._failed, self.reset_seed, reach=reach,
+                    first_env=self.first_env)
         self._failed_host.copy_(self._failed, non_blocking=True)
         self._failed_ev = torch.cuda.Event()
         self._failed_ev.record()
@@ -92,7 +98,7 @@ class VectorRollout:
         from ..env.device_reset import raise_on_failure
         self._failed_ev.synchronize()
         self._failed_ev = None
-        raise_on_failure(self.env, self._failed_host.numpy())
+        raise_on_failure(self.env, self._failed_host.numpy(), first_env=self.first_env)
 
     # ---- host side: initial conditions (the reference's rejection sampler, one env at a time) -------------------------
     def _sample_one(self):
@@ -271,9 +277,18 @@ def evaluate_episodes(env, algo, seeds: Sequence[int], rand: Optional[float] = 3
             live = live[stay]
     frac = lambda m: m.sum(dim=1).cpu().numpy() / n           # noqa: E731  (agent counts / n, as eval_ctrl_epi divides)
     res = {'reward': reward.cpu().numpy(), 'length': length, 'safe': frac(safe), 'reach': frac(reach), 'success': frac(safe & reach)}
-    stats = list(res.items())
-    res['mean'] = {k: float(np.mean(v)) for k, v in stats}
-    res['std'] = {k: float(np.std(v)) for k, v in stats}
-    res['final_states'] = final.cpu()
-    res['seeds'] = seeds
+    return episode_summary(res, final.cpu(), seeds)
+
+
+EPISODE_ARRAYS = ('reward', 'length', 'safe', 'reach', 'success')
+
+
+def episode_summary(per_episode: Dict[str, np.ndarray], final_states: torch.Tensor, seeds: Sequence[int]) -> Dict[str, object]:
+    """evaluate_episodes' result from its per-episode arrays (EPISODE_ARRAYS): the arrays, their `mean` / `std`, `final_states`
+    and `seeds`."""
+    res = {k: per_episode[k] for k in EPISODE_ARRAYS}
+    res['mean'] = {k: float(np.mean(res[k])) for k in EPISODE_ARRAYS}
+    res['std'] = {k: float(np.std(res[k])) for k in EPISODE_ARRAYS}
+    res['final_states'] = final_states
+    res['seeds'] = list(seeds)
     return res

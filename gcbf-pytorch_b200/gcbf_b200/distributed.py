@@ -8,9 +8,12 @@ GPUs over NVLink/NVSwitch, gloo in the CPU tests):
   2. all-gather of h_dot (M floats per rank, unequal shards allowed: sizes travel over a gloo companion group) + all-reduce
      of one int64 pair count   -> the M x M `acc/derivative` (gcbf.py:209) over the GLOBAL agent count
   3. ONE all-reduce (sum) of the flat fp32 gradient bucket of both nets (24.46 M floats)   -> clip + Adam (gcbf.py:220-226)
+The data-parallel vectorised Trainer adds host-side exchanges at evaluation only (broadcast of the episode seeds, gather of the
+per-episode results), on the same gloo companion group.
 """
 from typing import List, Optional, Tuple
 
+import numpy as np
 import torch
 
 
@@ -81,3 +84,25 @@ class Reducer:
         out = torch.empty(self.world, cap, device=t.device, dtype=t.dtype)
         self.dist.all_gather_into_tensor(out.view(-1), padded, group=self.group)
         return torch.cat([out[r, :n] for r, n in enumerate(sizes)])
+
+    # ---- host arrays (the vectorised Trainer's sharded evaluation), over the gloo companion group ---------------------------
+    def broadcast_host(self, a: np.ndarray) -> np.ndarray:
+        """Rank 0's array on every rank; every rank passes an array of the same shape and dtype."""
+        if self.world == 1:
+            return a
+        t = torch.from_numpy(np.array(a, copy=True))
+        self.dist.broadcast(t, group_src=0, group=self._host_group())
+        return t.numpy()
+
+    def gather_rows(self, a: np.ndarray, sizes: Optional[List[int]] = None) -> np.ndarray:
+        """Concatenation along axis 0 of every rank's array, in rank order.  Row counts may differ (`sizes`, from `sizes()`, or
+        exchanged here); the trailing shape and the dtype must be the same on every rank."""
+        if self.world == 1:
+            return a
+        sizes = self.sizes(a.shape[0]) if sizes is None else sizes
+        padded = np.zeros((max(sizes),) + a.shape[1:], dtype=a.dtype)
+        padded[:a.shape[0]] = a
+        mine = torch.from_numpy(padded)
+        out = [torch.empty_like(mine) for _ in range(self.world)]
+        self.dist.all_gather(out, mine, group=self._host_group())
+        return np.concatenate([o.numpy()[:n] for o, n in zip(out, sizes)])

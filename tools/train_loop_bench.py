@@ -9,7 +9,15 @@ Prints one JSON line per entry, and first the card's name and power limit (an ab
             128 done envs, SimpleCar at n = 16 and n = 64
   eval      Trainer.eval with 3 episodes one by one (algo.apply) against vectorised (evaluate_episodes), and vectorised with 32
 Envs: SimpleCar n = 16 and DubinsCar n = 16 with 8 obstacles (the reference's train.py defaults otherwise).  Nothing is written to the
-tree: checkpoints / summaries go to a temporary directory."""
+tree: checkpoints / summaries go to a temporary directory.
+
+Data-parallel mode, one process per rank: `torchrun --nproc-per-node R tools/train_loop_bench.py --dp [--intervals K]`.
+  dp        Trainer(num_envs=32) with algo.process_group on SimpleCar n = 256 in a 16 x 16 area (C2's env: one vector step is one
+            C2-sized batch of 32 graphs x 256 agents), batch_size = 512: one warm-up interval, then K intervals timed on every rank
+            (device synchronise, host clock; collection and updates).  Rank 0 prints per-rank and aggregate transitions/s (the
+            aggregate is all ranks' transitions over the slowest rank's wall time) with the rank count and each rank's card.  NCCL,
+            one GPU per rank (a rank's update at this size needs about 40 GB)."""
+import argparse
 import json
 import os
 import subprocess
@@ -35,13 +43,13 @@ DEV = torch.device('cuda:0')
 ENVS = [('SimpleCar', 16, {}), ('DubinsCar', 16, {'num_obs': 8})]
 
 
-def card():
+def card(index=0):
     try:
-        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
+        out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', str(index)],
                              capture_output=True, text=True, timeout=30).stdout.strip()
     except Exception as ex:
         out = f'nvidia-smi unavailable: {ex!r}'
-    return {'card': out or torch.cuda.get_device_name(0)}
+    return {'card': out or torch.cuda.get_device_name(index)}
 
 
 def emit(d):
@@ -142,8 +150,52 @@ def eval_leg(name, n, params):
                   'episodes': epi, 'wall_s': round(wall, 2), 'reward': round(reward, 3), **info})
 
 
+def dp_leg(intervals):
+    import torch.distributed as dist
+    rank, world = int(os.environ['RANK']), int(os.environ['WORLD_SIZE'])
+    local = int(os.environ.get('LOCAL_RANK', rank))
+    assert local < torch.cuda.device_count(), f'--dp needs one GPU per rank: local rank {local}, {torch.cuda.device_count()} GPU(s)'
+    dev = torch.device('cuda', local)
+    torch.cuda.set_device(dev)
+    dist.init_process_group('nccl', device_id=dev)
+    try:
+        name, n, params, num_envs = 'SimpleCar', 256, {'area_size': 16.0}, 32
+        set_seed(0)
+        env, algo = seeded_algo(name, n, dev, 0, params)
+        env_test = make_env(name, n, dev, params=env._params)
+        algo.process_group = dist.group.WORLD
+        with tempfile.TemporaryDirectory() as tmp:
+            tr = Trainer(env, env_test, algo, tmp, num_envs=num_envs, seed=0)
+            tr.train(algo.batch_size, 0, 0)                    # warm-up interval (also fills memory, as a running job has)
+            torch.cuda.synchronize()
+            dist.barrier()
+            t0 = time.perf_counter()
+            tr.train(intervals * algo.batch_size, 0, 0)
+            torch.cuda.synchronize()
+            wall = time.perf_counter() - t0
+        red = algo._reducer()
+        walls = red.gather_rows(np.array([wall]))
+        mine = np.frombuffer(card(dev.index)['card'].encode()[:200].ljust(200), dtype=np.uint8)[None]
+        cards = [bytes(row).decode().strip() for row in red.gather_rows(mine)]
+        if rank == 0:
+            per_rank = intervals * algo.batch_size
+            emit({'leg': 'dp', 'env': name, 'n': n, 'area_size': params['area_size'], 'num_envs_per_rank': num_envs,
+                  'batch_size': algo.batch_size, 'ranks': world,
+                  'cards': cards, 'intervals': intervals, 'wall_s': [round(float(w), 3) for w in walls],
+                  'transitions_per_s_per_rank': [round(per_rank / float(w), 0) for w in walls],
+                  'transitions_per_s_aggregate': round(world * per_rank / float(walls.max()), 0)})
+    finally:
+        dist.destroy_process_group()
+
+
 def main():
     assert torch.cuda.is_available(), 'train_loop_bench needs a GPU'
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--dp', action='store_true', help='data-parallel mode, one process per rank under torchrun')
+    ap.add_argument('--intervals', type=int, default=3, help='timed update intervals per rank in --dp mode')
+    args = ap.parse_args()
+    if args.dp:
+        return dp_leg(args.intervals)
     emit(card())
     for name, n, params in ENVS:
         interval_leg(name, n, params)
