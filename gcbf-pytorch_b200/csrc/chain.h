@@ -48,17 +48,11 @@ struct Run {
   } while (0)
 #define CHAIN_CUDA(expr) GCBF_CUDA_OK(expr)
 
-// fp16 [hi | lo] companion of an fp32 matrix (gemm_wgmma_f16.cu)
-struct H16 {
-  void* buf; const void* amax; int ld, rows, cols;
-  int sr, sc;   // strides (words) of the amax array per 128-row block / 256-column tile; 0, 0 = one word per tensor
-};
-
 struct MlpCtx {
   int n, M;
   const float* acts[GCBF_MAX_MLP_LAYERS + 1];   // acts[0] = input, acts[l + 1] = output of layer l
   int ld[GCBF_MAX_MLP_LAYERS + 1];
-  H16 acts_h[GCBF_MAX_MLP_LAYERS];               // companion of acts[l] when layer l ran on the tensor cores (buf == nullptr otherwise)
+  gcbf_h16 acts_h[GCBF_MAX_MLP_LAYERS];          // companion of acts[l] when layer l ran on the tensor cores (buf == nullptr otherwise)
   const float* inv_sigma[GCBF_MAX_MLP_LAYERS];
   const float* u[GCBF_MAX_MLP_LAYERS];           // spectral-norm vectors of THIS forward (snapshots)
   const float* v[GCBF_MAX_MLP_LAYERS];

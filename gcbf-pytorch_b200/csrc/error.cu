@@ -13,7 +13,7 @@ void set_error(const char* fmt, ...) {
 }  // namespace gcbf
 
 extern "C" const char* gcbf_last_error(void) { return gcbf::g_err; }
-extern "C" int gcbf_abi_version(void) { return 5; }   // 2: fp16-companion tensor-core entry points (gcbf_linear_*_h); 3: chain-level entry points (gcbf_net_*, gcbf_mlp_*, gcbf_step_*); 4: + MACBF kernels (macbf.cu) and the analytic h_dot kernels (jvp.cu), nothing removed; 5: sm_90a build, gcbf_has_tcgen05 renamed gcbf_has_wgmma; later additions within 5 (nothing changed or removed): gcbf_apply_batch + gcbf_apply_batch_workspace_bytes, gcbf_cbf_field + gcbf_cbf_field_workspace_bytes (gcbf_field_desc), gcbf_env_reset_batch (gcbf_reset_desc)
+extern "C" int gcbf_abi_version(void) { return 6; }   // 2: fp16-companion tensor-core entry points (gcbf_linear_*_h); 3: chain-level entry points (gcbf_net_*, gcbf_mlp_*, gcbf_step_*); 4: + MACBF kernels (macbf.cu) and the analytic h_dot kernels (jvp.cu), nothing removed; 5: sm_90a build, gcbf_has_tcgen05 renamed gcbf_has_wgmma; later additions within 5 (nothing changed or removed): gcbf_apply_batch + gcbf_apply_batch_workspace_bytes, gcbf_cbf_field + gcbf_cbf_field_workspace_bytes (gcbf_field_desc), gcbf_env_reset_batch (gcbf_reset_desc); 6: gcbf_linear_*_h take gcbf_h16 descriptors and `products` (the raw-pointer signatures and gcbf_linear_*_t / _tp are gone)
 
 // sizeof() of the ABI structures as this library was compiled (bindings check their mirrors against it):
 // 0 gcbf_env_cfg, 1 gcbf_linear_desc, 2 gcbf_net_desc, 3 gcbf_step_desc, 4 gcbf_step_batch, 5 gcbf_step_out, 6 gcbf_net_ctx,

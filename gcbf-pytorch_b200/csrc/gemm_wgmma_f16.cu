@@ -916,13 +916,13 @@ static int check_h16(const gcbf_h16* h, const char* what, int rows, int cols) {
 
 // Y[M,N] = act(alpha * X W^T + bias): A = X companion [M][K] (K-major), B = W companion [N][K] (K-major, per-tensor scale).
 // products: 3 (3xFP16) or 1 (fp16: the hi planes only; the companions keep their [hi|lo] format)
-extern "C" int gcbf_linear_fwd_tp(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
-                                  const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream, int products) {
-  GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && (Y || Yh) && (!Y || ldy >= N), "gcbf_linear_fwd_t: bad arguments M=%d N=%d K=%d", M, N, K);
-  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_fwd_tp: products %d (3 or 1)", products);
-  if (int rc = check_h16(X, "gcbf_linear_fwd_t X", M, K)) return rc;
-  if (int rc = check_h16(W, "gcbf_linear_fwd_t W", N, K)) return rc;
-  GCBF_REQUIRE(W->amax_row_stride == 0 && W->amax_col_stride == 0, "gcbf_linear_fwd_t: the weight companion must be per-tensor scaled");
+extern "C" int gcbf_linear_fwd_h(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
+                                 const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream, int products) {
+  GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && (Y || Yh) && (!Y || ldy >= N), "gcbf_linear_fwd_h: bad arguments M=%d N=%d K=%d", M, N, K);
+  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_fwd_h: products %d (3 or 1)", products);
+  if (int rc = check_h16(X, "gcbf_linear_fwd_h X", M, K)) return rc;
+  if (int rc = check_h16(W, "gcbf_linear_fwd_h W", N, K)) return rc;
+  GCBF_REQUIRE(W->amax_row_stride == 0 && W->amax_col_stride == 0, "gcbf_linear_fwd_h: the weight companion must be per-tensor scaled");
   cudaStream_t st = as_stream(stream);
   th::EpiParams ep{};
   ep.mode = th::EPI_FWD; ep.alpha = inv_sigma; ep.bias = bias; ep.act = act;
@@ -932,8 +932,8 @@ extern "C" int gcbf_linear_fwd_tp(const gcbf_h16* X, const gcbf_h16* W, const fl
   if (out_amax) GCBF_CUDA_OK(cudaMemsetAsync(out_amax, 0, 4, st));
   th::OutH oh{};
   if (Yh) {
-    if (int rc = check_h16(Yh, "gcbf_linear_fwd_t Yh", M, N)) return rc;
-    GCBF_REQUIRE(N > 128 && Yh->amax_row_stride == ceil_div(N, 256) && Yh->amax_col_stride == 1, "gcbf_linear_fwd_t: emitted companions are tile-scaled (N > 128, amax strides (ceil(N/256), 1))");
+    if (int rc = check_h16(Yh, "gcbf_linear_fwd_h Yh", M, N)) return rc;
+    GCBF_REQUIRE(N > 128 && Yh->amax_row_stride == ceil_div(N, 256) && Yh->amax_col_stride == 1, "gcbf_linear_fwd_h: emitted companions are tile-scaled (N > 128, amax strides (ceil(N/256), 1))");
     oh = th::OutH{reinterpret_cast<__half*>(Yh->buf), M, N, Yh->ld, reinterpret_cast<uint32_t*>(Yh->amax), Yh->amax_row_stride};
   }
   th::Operand A{reinterpret_cast<const __half*>(X->buf), M, K, X->ld, false}, B{reinterpret_cast<const __half*>(W->buf), N, K, W->ld, false};
@@ -941,23 +941,18 @@ extern "C" int gcbf_linear_fwd_tp(const gcbf_h16* X, const gcbf_h16* W, const fl
                    : th::launch_p<128, false, false>(products, A, B, Y, ldy, M, N, K, 1, ep, nullptr, st);
 }
 
-extern "C" int gcbf_linear_fwd_t(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
-                                 const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream) {
-  return gcbf_linear_fwd_tp(X, W, bias, inv_sigma, act, Y, ldy, Yh, out_amax, M, N, K, stream, 3);
-}
-
 // dX[M,K] (+)= alpha * dZ W (* relu mask): A = dZ companion [M][N] (K-major: contraction over N), B = W companion [N][K] (MN-major)
-extern "C" int gcbf_linear_bwd_data_tp(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
-                                       const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
-                                       void* out_amax, int M, int N, int K, void* stream, int products) {
-  GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && (dX || dXh) && (!dX || lddx >= K), "gcbf_linear_bwd_data_t: bad arguments M=%d N=%d K=%d", M, N, K);
-  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_bwd_data_tp: products %d (3 or 1)", products);
-  GCBF_REQUIRE(!relu_src || ld_relu >= K, "gcbf_linear_bwd_data_t: ld_relu");
-  GCBF_REQUIRE(!(relu_src && relu_h) && !(accumulate && (dXh || colsum)), "gcbf_linear_bwd_data_t: conflicting options");
-  if (int rc = check_h16(dZ, "gcbf_linear_bwd_data_t dZ", M, N)) return rc;
-  if (int rc = check_h16(W, "gcbf_linear_bwd_data_t W", N, K)) return rc;
-  GCBF_REQUIRE(W->amax_row_stride == 0 && W->amax_col_stride == 0, "gcbf_linear_bwd_data_t: the weight companion must be per-tensor scaled");
-  if (relu_h) { if (int rc = check_h16(relu_h, "gcbf_linear_bwd_data_t relu_h", M, K)) return rc; }
+extern "C" int gcbf_linear_bwd_data_h(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
+                                      const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
+                                      void* out_amax, int M, int N, int K, void* stream, int products) {
+  GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && (dX || dXh) && (!dX || lddx >= K), "gcbf_linear_bwd_data_h: bad arguments M=%d N=%d K=%d", M, N, K);
+  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_bwd_data_h: products %d (3 or 1)", products);
+  GCBF_REQUIRE(!relu_src || ld_relu >= K, "gcbf_linear_bwd_data_h: ld_relu");
+  GCBF_REQUIRE(!(relu_src && relu_h) && !(accumulate && (dXh || colsum)), "gcbf_linear_bwd_data_h: conflicting options");
+  if (int rc = check_h16(dZ, "gcbf_linear_bwd_data_h dZ", M, N)) return rc;
+  if (int rc = check_h16(W, "gcbf_linear_bwd_data_h W", N, K)) return rc;
+  GCBF_REQUIRE(W->amax_row_stride == 0 && W->amax_col_stride == 0, "gcbf_linear_bwd_data_h: the weight companion must be per-tensor scaled");
+  if (relu_h) { if (int rc = check_h16(relu_h, "gcbf_linear_bwd_data_h relu_h", M, K)) return rc; }
   cudaStream_t st = as_stream(stream);
   th::EpiParams ep{};
   ep.mode = th::EPI_DGRAD; ep.alpha = inv_sigma; ep.relu_src = relu_src; ep.ld_relu = ld_relu; ep.accumulate = accumulate;
@@ -969,8 +964,8 @@ extern "C" int gcbf_linear_bwd_data_tp(const gcbf_h16* dZ, const gcbf_h16* W, co
   if (out_amax) GCBF_CUDA_OK(cudaMemsetAsync(out_amax, 0, 4, st));
   th::OutH oh{};
   if (dXh) {
-    if (int rc = check_h16(dXh, "gcbf_linear_bwd_data_t dXh", M, K)) return rc;
-    GCBF_REQUIRE(K > 128 && dXh->amax_row_stride == ceil_div(K, 256) && dXh->amax_col_stride == 1, "gcbf_linear_bwd_data_t: emitted companions are tile-scaled (K > 128, amax strides (ceil(K/256), 1))");
+    if (int rc = check_h16(dXh, "gcbf_linear_bwd_data_h dXh", M, K)) return rc;
+    GCBF_REQUIRE(K > 128 && dXh->amax_row_stride == ceil_div(K, 256) && dXh->amax_col_stride == 1, "gcbf_linear_bwd_data_h: emitted companions are tile-scaled (K > 128, amax strides (ceil(K/256), 1))");
     oh = th::OutH{reinterpret_cast<__half*>(dXh->buf), M, K, dXh->ld, reinterpret_cast<uint32_t*>(dXh->amax), dXh->amax_row_stride};
   }
   th::Operand A{reinterpret_cast<const __half*>(dZ->buf), M, N, dZ->ld, false}, B{reinterpret_cast<const __half*>(W->buf), N, K, W->ld, true};
@@ -978,19 +973,13 @@ extern "C" int gcbf_linear_bwd_data_tp(const gcbf_h16* dZ, const gcbf_h16* W, co
                    : th::launch_p<128, false, true>(products, A, B, dX, lddx, M, K, N, 1, ep, nullptr, st);
 }
 
-extern "C" int gcbf_linear_bwd_data_t(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
-                                      const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
-                                      void* out_amax, int M, int N, int K, void* stream) {
-  return gcbf_linear_bwd_data_tp(dZ, W, inv_sigma, relu_src, ld_relu, relu_h, dX, lddx, accumulate, dXh, colsum, out_amax, M, N, K, stream, 3);
-}
-
 // dW[N,K] (+)= alpha * dZ^T X: A = dZ companion [M][N] (MN-major), B = X companion [M][K] (MN-major); contraction over M
-extern "C" int gcbf_linear_bwd_weight_tp(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
-                                         int M, int N, int K, void* stream, int products) {
-  GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && lddw >= K && dW, "gcbf_linear_bwd_weight_t: bad arguments M=%d N=%d K=%d", M, N, K);
-  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_bwd_weight_tp: products %d (3 or 1)", products);
-  if (int rc = check_h16(dZ, "gcbf_linear_bwd_weight_t dZ", M, N)) return rc;
-  if (int rc = check_h16(X, "gcbf_linear_bwd_weight_t X", M, K)) return rc;
+extern "C" int gcbf_linear_bwd_weight_h(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
+                                        int M, int N, int K, void* stream, int products) {
+  GCBF_REQUIRE(M > 0 && N > 0 && K > 0 && lddw >= K && dW, "gcbf_linear_bwd_weight_h: bad arguments M=%d N=%d K=%d", M, N, K);
+  GCBF_REQUIRE(products == 3 || products == 1, "gcbf_linear_bwd_weight_h: products %d (3 or 1)", products);
+  if (int rc = check_h16(dZ, "gcbf_linear_bwd_weight_h dZ", M, N)) return rc;
+  if (int rc = check_h16(X, "gcbf_linear_bwd_weight_h X", M, K)) return rc;
   cudaStream_t st = as_stream(stream);
   th::EpiParams ep{};
   ep.mode = th::EPI_WGRAD; ep.alpha = inv_sigma; ep.accumulate = accumulate;
@@ -1003,40 +992,4 @@ extern "C" int gcbf_linear_bwd_weight_tp(const gcbf_h16* dZ, const gcbf_h16* X, 
   th::Operand A{reinterpret_cast<const __half*>(dZ->buf), M, N, dZ->ld, true}, B{reinterpret_cast<const __half*>(X->buf), M, K, X->ld, true};
   return (BN == 256) ? th::launch_p<256, true, true>(products, A, B, dW, lddw, N, K, M, splits, ep, nullptr, st)
                      : th::launch_p<128, true, true>(products, A, B, dW, lddw, N, K, M, splits, ep, nullptr, st);
-}
-
-extern "C" int gcbf_linear_bwd_weight_t(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
-                                        int M, int N, int K, void* stream) {
-  return gcbf_linear_bwd_weight_tp(dZ, X, inv_sigma, dW, lddw, accumulate, M, N, K, stream, 3);
-}
-
-// ---- the per-tensor-scaled entry points of ABI v2: thin wrappers ------------------------------------------------------------------------
-static gcbf_h16 per_tensor(const void* buf, int ld, const void* amax, int rows, int cols) {
-  gcbf_h16 h;
-  h.buf = const_cast<void*>(buf); h.amax = const_cast<void*>(amax); h.ld = ld; h.rows = rows; h.cols = cols; h.amax_row_stride = 0; h.amax_col_stride = 0;
-  return h;
-}
-
-extern "C" int gcbf_linear_fwd_h(const void* Xh, int ldxh, const void* x_amax, const void* Wh, int ldwh, const void* w_amax,
-                                 const float* bias, const float* inv_sigma, float* Y, int ldy, int M, int N, int K, int act,
-                                 void* out_amax, void* stream) {
-  GCBF_REQUIRE(Y && x_amax && w_amax, "gcbf_linear_fwd_h: null pointer");
-  const gcbf_h16 X = per_tensor(Xh, ldxh, x_amax, M, K), W = per_tensor(Wh, ldwh, w_amax, N, K);
-  return gcbf_linear_fwd_t(&X, &W, bias, inv_sigma, act, Y, ldy, nullptr, out_amax, M, N, K, stream);
-}
-
-extern "C" int gcbf_linear_bwd_data_h(const void* dZh, int lddzh, const void* dz_amax, const void* Wh, int ldwh,
-                                      const void* w_amax, const float* inv_sigma, const float* relu_src, int ld_relu, float* dX,
-                                      int lddx, int M, int N, int K, int accumulate, void* out_amax, void* stream) {
-  GCBF_REQUIRE(dX && dz_amax && w_amax, "gcbf_linear_bwd_data_h: null pointer");
-  const gcbf_h16 dZ = per_tensor(dZh, lddzh, dz_amax, M, N), W = per_tensor(Wh, ldwh, w_amax, N, K);
-  return gcbf_linear_bwd_data_t(&dZ, &W, inv_sigma, relu_src, ld_relu, nullptr, dX, lddx, accumulate, nullptr, nullptr, out_amax, M, N, K, stream);
-}
-
-extern "C" int gcbf_linear_bwd_weight_h(const void* dZh, int lddzh, const void* dz_amax, const void* Xh, int ldxh,
-                                        const void* x_amax, const float* inv_sigma, float* dW, int lddw, int M, int N, int K,
-                                        int accumulate, void* stream) {
-  GCBF_REQUIRE(dW && dz_amax && x_amax, "gcbf_linear_bwd_weight_h: null pointer");
-  const gcbf_h16 dZ = per_tensor(dZh, lddzh, dz_amax, M, N), X = per_tensor(Xh, ldxh, x_amax, M, K);
-  return gcbf_linear_bwd_weight_t(&dZ, &X, inv_sigma, dW, lddw, accumulate, M, N, K, stream);
 }

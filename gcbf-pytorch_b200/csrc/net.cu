@@ -47,13 +47,13 @@ struct Timed {
 // ---- operand preparation -------------------------------------------------------------------------------------------
 // amax (unless the producer supplied it) + fp16 [hi|lo] split of x[rows, cols] (pitch ld); optional column sums into `colsum`
 // (accumulated: it is a bias's gradient target)
-int split_h(Run& R, const float* x, int ld, int rows, int cols, const void* amax, float* colsum, H16* out) {
+int split_h(Run& R, const float* x, int ld, int rows, int cols, const void* amax, float* colsum, gcbf_h16* out) {
   const int ld_h = (cols + 7) / 8 * 8;
   out->buf = R.ws.alloc((size_t)2 * rows * ld_h * 2);
-  out->ld = ld_h; out->rows = rows; out->cols = cols; out->sr = 0; out->sc = 0;
+  out->ld = ld_h; out->rows = rows; out->cols = cols; out->amax_row_stride = 0; out->amax_col_stride = 0;
   void* own = nullptr;
   if (!amax) own = R.amax_slot();
-  out->amax = amax ? amax : own;
+  out->amax = amax ? const_cast<void*>(amax) : own;   // a producer's word: only read from here on
   if (R.dry) return 0;
   Timed t(R, 4, 0.0, rows, cols, 0);
   if (!amax) { CHAIN_CALL(gcbf_amax_f32(x, ld, rows, cols, own, 0, R.st)); R.launched(1); }
@@ -143,24 +143,18 @@ static bool epi_h_enabled() {
 static bool can_emit(int M, int width, int consumer_n) { return epi_h_enabled() && width > 128 && consumer_n > 0 && use_h(M, consumer_n, width); }
 static bool can_emit_bwd(int M, int width, int consumer_n) { return can_emit(M, width, consumer_n) && g_epi_h_bwd == 1; }
 
-static gcbf_h16 h16_desc(const H16& h) {
-  gcbf_h16 d;
-  d.buf = h.buf; d.amax = const_cast<void*>(h.amax); d.ld = h.ld; d.rows = h.rows; d.cols = h.cols;
-  d.amax_row_stride = h.sr; d.amax_col_stride = h.sc; d.pad_ = 0;
-  return d;
-}
 static gcbf_h16 weight_desc(const gcbf_linear_desc& L) {
-  gcbf_h16 d;
-  d.buf = L.Wh; d.amax = L.w_amax; d.ld = L.ldwh; d.rows = L.N; d.cols = L.K; d.amax_row_stride = 0; d.amax_col_stride = 0; d.pad_ = 0;
+  gcbf_h16 d{};
+  d.buf = L.Wh; d.amax = L.w_amax; d.ld = L.ldwh; d.rows = L.N; d.cols = L.K;
   return d;
 }
 // buffers of a tile-scaled companion an epilogue is about to write
-static H16 alloc_tiled(Run& R, int rows, int cols) {
-  H16 h{};
+static gcbf_h16 alloc_tiled(Run& R, int rows, int cols) {
+  gcbf_h16 h{};
   h.ld = (cols + 7) / 8 * 8; h.rows = rows; h.cols = cols;
   h.buf = R.ws.alloc((size_t)2 * rows * h.ld * 2);
-  h.sr = (cols + 255) / 256; h.sc = 1;
-  h.amax = R.ws.alloc((size_t)((rows + 127) / 128) * h.sr * 4);
+  h.amax_row_stride = (cols + 255) / 256; h.amax_col_stride = 1;
+  h.amax = R.ws.alloc((size_t)((rows + 127) / 128) * h.amax_row_stride * 4);
   return h;
 }
 
@@ -169,15 +163,15 @@ static H16 alloc_tiled(Run& R, int rows, int cols) {
 // `out`: where the LAST layer writes its fp32 output (pitch ld_out), or nullptr for a workspace buffer; out_h (optional): receives the
 // emitted companion of the output when the consumer qualifies (buf == nullptr otherwise) -- the fp32 output is then written only
 // if need_f32_out.
-int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, int ldx, int M, const H16* x_h, const void* x_amax,
+int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, int ldx, int M, const gcbf_h16* x_h, const void* x_amax,
                 int next_width, const float* const* inv_sigma, const float* const* us, const float* const* vs, MlpCtx* ctx, float* out,
-                int ld_out, bool need_f32_out, H16* out_h, const float** y, int* ldy, const void** y_amax, int products) {
+                int ld_out, bool need_f32_out, gcbf_h16* out_h, const float** y, int* ldy, const void** y_amax, int products) {
   if (ctx) { memset(ctx, 0, sizeof(*ctx)); ctx->n = n; ctx->M = M; ctx->acts[0] = x; ctx->ld[0] = ldx; }
   const float* cur = x;
   int ldc = ldx;
-  H16 cur_h = x_h ? *x_h : H16{};
+  gcbf_h16 cur_h = x_h ? *x_h : gcbf_h16{};
   const void* cur_amax = x_amax;
-  if (out_h) *out_h = H16{};
+  if (out_h) *out_h = gcbf_h16{};
   for (int l = 0; l < n; ++l) {
     const gcbf_linear_desc& L = layers[l];
     const int N = L.N, K = L.K;
@@ -193,15 +187,15 @@ int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, i
       if (lastl && out) { dst = out; ldd = ld_out; }
       else dst = (float*)R.ws.alloc((size_t)M * N * 4);
     }
-    H16 yh{};
+    gcbf_h16 yh{};
     if (h) {
       if (!L.Wh) { set_error("layer [%d x %d] runs on the tensor cores but its descriptor has no weight companion", N, K); return GCBF_E_INVALID; }
       if (!cur_h.buf) { if (int rc = split_h(R, cur, ldc, M, K, cur_amax, nullptr, &cur_h)) return rc; }
       if (emit) yh = alloc_tiled(R, M, N);
       if (!R.dry) {
         Timed t(R, 0, 2.0 * M * N * K, M, N, K);
-        const gcbf_h16 X = h16_desc(cur_h), W = weight_desc(L), Y = h16_desc(yh);
-        CHAIN_CALL(gcbf_linear_fwd_tp(&X, &W, L.b, inv_sigma[l], L.act, dst, ldd, emit ? &Y : nullptr, ya, M, N, K, R.st, products));
+        const gcbf_h16 W = weight_desc(L);
+        CHAIN_CALL(gcbf_linear_fwd_h(&cur_h, &W, L.b, inv_sigma[l], L.act, dst, ldd, emit ? &yh : nullptr, ya, M, N, K, R.st, products));
         R.launched(1);
       }
     } else if (sk_emit) {
@@ -209,8 +203,7 @@ int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, i
       yh = alloc_tiled(R, M, N);
       if (!R.dry) {
         Timed t(R, 3, 2.0 * M * N * K, M, N, K);
-        const gcbf_h16 Y = h16_desc(yh);
-        CHAIN_CALL(gcbf_linear_fwd_emit(cur, ldc, L.W, L.ldw, L.b, inv_sigma[l], L.act, &Y, M, N, K, R.st));
+        CHAIN_CALL(gcbf_linear_fwd_emit(cur, ldc, L.W, L.ldw, L.b, inv_sigma[l], L.act, &yh, M, N, K, R.st));
         R.launched(1);
       }
     } else {
@@ -223,7 +216,7 @@ int mlp_forward(Run& R, const gcbf_linear_desc* layers, int n, const float* x, i
     }
     if (ctx) {
       ctx->acts[l + 1] = dst; ctx->ld[l + 1] = ldd;
-      ctx->acts_h[l] = h ? cur_h : H16{};
+      ctx->acts_h[l] = h ? cur_h : gcbf_h16{};
       ctx->inv_sigma[l] = inv_sigma[l]; ctx->u[l] = us[l]; ctx->v[l] = vs[l];
     }
     cur = dst; ldc = ldd; cur_amax = ya; cur_h = yh;
@@ -252,17 +245,17 @@ int vec_add(Run& R, float* dst, const float* src, int64_t n) {
 // buffer; dx_amax: word that receives max|dx| if the input-gradient GEMM runs on the tensor cores (*dx_amax_valid).  dx_h (optional):
 // the caller's consumer is a tensor-core layer with `dx_consumer_n` outputs whose bias gradient lives at dx_colsum: if the producer
 // qualifies, dx is emitted as a companion only (*dx == nullptr, dx_h->buf != nullptr) and its column sums are added to dx_colsum.
-int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ctx, const float* dy, int ld_dy, const H16* dy_h,
+int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ctx, const float* dy, int ld_dy, const gcbf_h16* dy_h,
                  bool dy_colsum_done, bool need_dx, float* dx_out, int ld_dx, bool dx_accumulate, const void* dy_amax, void* dx_amax,
-                 bool skip_wgrad, H16* dx_h, int dx_consumer_n, float* dx_colsum, const float** dx, int* ld_dx_res, bool* dx_amax_valid,
+                 bool skip_wgrad, gcbf_h16* dx_h, int dx_consumer_n, float* dx_colsum, const float** dx, int* ld_dx_res, bool* dx_amax_valid,
                  int products) {
   const int M = ctx.M;
   const int last = n - 1;
   const float* dz = dy;
   int lddz = ld_dy;
-  H16 dzh = dy_h ? *dy_h : H16{};
+  gcbf_h16 dzh = dy_h ? *dy_h : gcbf_h16{};
   bool colsum_done = dy_h ? dy_colsum_done : false;
-  if (dx_h) *dx_h = H16{};
+  if (dx_h) *dx_h = gcbf_h16{};
   if (layers[last].act != GCBF_ACT_NONE) {
     const int N = layers[last].N;
     if (!dz || ld_dy != N || ctx.ld[last + 1] != N || !ctx.acts[last + 1]) { set_error("mlp_backward: output activation needs dense fp32 d_out / output"); return GCBF_E_INVALID; }
@@ -287,28 +280,26 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
       } else if (wgrad && L.gb && !colsum_done) {
         set_error("mlp_backward: emitted gradient companion without its bias gradient"); return GCBF_E_INVALID;
       }
-      const gcbf_h16 dZ = h16_desc(dzh), W = weight_desc(L);
+      const gcbf_h16 W = weight_desc(L);
       if (wgrad) {
-        H16 xh = ctx.acts_h[l];
+        gcbf_h16 xh = ctx.acts_h[l];
         if (!xh.buf) { if (int rc = split_h(R, x_in, ldx, M, K, nullptr, nullptr, &xh)) return rc; }
-        const gcbf_h16 X = h16_desc(xh);
         if (L.u) {
           float* dW = (float*)R.ws.alloc((size_t)N * K * 4);
           float* fx = (float*)R.ws.alloc(gcbf_sn_workspace_floats(N, K) * 4);
           if (!R.dry) {
             { Timed t(R, 2, 2.0 * M * N * K, M, N, K);
-              CHAIN_CALL(gcbf_linear_bwd_weight_tp(&dZ, &X, isg, dW, K, 0, M, N, K, R.st, products)); }
+              CHAIN_CALL(gcbf_linear_bwd_weight_h(&dzh, &xh, isg, dW, K, 0, M, N, K, R.st, products)); }
             CHAIN_CALL(gcbf_sn_grad_fixup(dW, K, L.W, L.ldw, N, K, ctx.u[l], ctx.v[l], isg, fx, L.gW, L.ldgw, R.st));
             R.launched(3);
           }
         } else if (!R.dry) {
           Timed t(R, 2, 2.0 * M * N * K, M, N, K);
-          CHAIN_CALL(gcbf_linear_bwd_weight_tp(&dZ, &X, isg, L.gW, L.ldgw, 1, M, N, K, R.st, products));
+          CHAIN_CALL(gcbf_linear_bwd_weight_h(&dzh, &xh, isg, L.gW, L.ldgw, 1, M, N, K, R.st, products));
           R.launched(1);
         }
       }
       // ReLU mask of the layer below: from its fp32 output, or from the hi plane of that output's companion
-      const gcbf_h16 maskh = h16_desc(ctx.acts_h[l]);
       const bool mask_h = (x_in == nullptr);
       if (l > 0) {
         const gcbf_linear_desc& P = layers[l - 1];
@@ -316,13 +307,12 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
         const bool pw = !skip_wgrad && P.gW && P.gb;
         void* na = (!emit && use_h(M, K, P.K)) ? R.amax_slot() : nullptr;
         float* o = emit ? nullptr : (float*)R.ws.alloc((size_t)M * K * 4);
-        H16 oh{};
+        gcbf_h16 oh{};
         if (emit) oh = alloc_tiled(R, M, K);
         if (!R.dry) {
           Timed t(R, 1, 2.0 * M * N * K, M, N, K);
-          const gcbf_h16 O = h16_desc(oh);
-          CHAIN_CALL(gcbf_linear_bwd_data_tp(&dZ, &W, isg, mask_h ? nullptr : x_in, ldx, mask_h ? &maskh : nullptr, o, K, 0, emit ? &O : nullptr,
-                                             (emit && pw) ? P.gb : nullptr, na, M, N, K, R.st, products));
+          CHAIN_CALL(gcbf_linear_bwd_data_h(&dzh, &W, isg, mask_h ? nullptr : x_in, ldx, mask_h ? &ctx.acts_h[l] : nullptr, o, K, 0, emit ? &oh : nullptr,
+                                            (emit && pw) ? P.gb : nullptr, na, M, N, K, R.st, products));
           R.launched(1);
         }
         dz = o; lddz = K; dz_amax = na; dzh = oh; colsum_done = emit && pw;
@@ -330,13 +320,12 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
         const bool emit = dx_h && !dx_out && !dx_accumulate && can_emit_bwd(M, K, dx_consumer_n);
         float* o = dx_out; int ldo = ld_dx;
         if (!o && !emit) { o = (float*)R.ws.alloc((size_t)M * K * 4); ldo = K; }
-        H16 oh{};
+        gcbf_h16 oh{};
         if (emit) oh = alloc_tiled(R, M, K);
         if (!R.dry) {
           Timed t(R, 1, 2.0 * M * N * K, M, N, K);
-          const gcbf_h16 O = h16_desc(oh);
-          CHAIN_CALL(gcbf_linear_bwd_data_tp(&dZ, &W, isg, nullptr, 0, nullptr, o, ldo, dx_accumulate ? 1 : 0, emit ? &O : nullptr,
-                                             (emit && !skip_wgrad) ? dx_colsum : nullptr, emit ? nullptr : dx_amax, M, N, K, R.st, products));
+          CHAIN_CALL(gcbf_linear_bwd_data_h(&dzh, &W, isg, nullptr, 0, nullptr, o, ldo, dx_accumulate ? 1 : 0, emit ? &oh : nullptr,
+                                            (emit && !skip_wgrad) ? dx_colsum : nullptr, emit ? nullptr : dx_amax, M, N, K, R.st, products));
           R.launched(1);
         }
         dz = o; lddz = ldo;
@@ -350,7 +339,7 @@ int mlp_backward(Run& R, const gcbf_linear_desc* layers, int n, const MlpCtx& ct
     }
     if (!dz && M > 0) { set_error("mlp_backward: layer %d needs its fp32 output gradient", l); return GCBF_E_INVALID; }
     dz_amax = nullptr;
-    dzh = H16{};
+    dzh = gcbf_h16{};
     const int impl = g_gemm_impl == 1 ? 1 : 0;
     if (wgrad) {
       if (L.u) {
@@ -467,7 +456,7 @@ int net_forward(Run& R, const gcbf_net_desc& net, const float* x, const float* e
   const float *msg, *gate, *feat;
   int ldm, ldg, ldf;
   const void *msg_amax = nullptr, *feat_amax = nullptr;
-  H16 msg_h{}, feat_h{};
+  gcbf_h16 msg_h{}, feat_h{};
   // phi's output is needed twice: as fp32 by the aggregation and (as a companion, when the gate's first layer is a tensor-core
   // layer) by gate_nn -- the last phi layer writes both
   if (int rc = mlp_forward(R, net.phi, net.n_phi, ein, kin, E, nullptr, nullptr, net.gate[0].N, isg, us, vs, save ? &ctx->phi : nullptr, nullptr, 0,
@@ -523,7 +512,7 @@ int net_backward(Run& R, const gcbf_net_desc& net, const NetCtx& ctx, const int3
   const float* d_feat = d_out;
   int ld_dfeat = ld_dout;
   const void* d_feat_amax = nullptr;
-  H16 d_feat_h{};
+  gcbf_h16 d_feat_h{};
   const gcbf_linear_desc& GL = net.gamma[net.n_gamma - 1];
   const bool g_colsum = !skip_wgrad && GL.gW && GL.gb;
   if (net.n_head > 0) {

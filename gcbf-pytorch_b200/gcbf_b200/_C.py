@@ -62,9 +62,6 @@ _SIGS = {
     'gcbf_split_f16': (c_int, [P, c_int, c_int, c_int, P, P, c_int, P, c_int, P]),
     'gcbf_amax_split_batched': (c_int, [POINTER(SplitDesc), c_int, P]),
     'gcbf_linear_h_supported': (c_int, [c_int, c_int, c_int]),
-    'gcbf_linear_fwd_h': (c_int, [P, c_int, P, P, c_int, P, P, P, P, c_int, c_int, c_int, c_int, c_int, P, P]),
-    'gcbf_linear_bwd_data_h': (c_int, [P, c_int, P, P, c_int, P, P, P, c_int, P, c_int, c_int, c_int, c_int, c_int, P, P]),
-    'gcbf_linear_bwd_weight_h': (c_int, [P, c_int, P, P, c_int, P, P, P, c_int, c_int, c_int, c_int, c_int, P]),
     'gcbf_act_bwd': (c_int, [P, P, P, c_int64, c_int, P]),
     'gcbf_attn_aggr_fwd': (c_int, [P, c_int, P, P, c_int, c_int, P, P, c_int, P]),
     'gcbf_attn_aggr_bwd': (c_int, [P, c_int, P, P, c_int, c_int, P, c_int, P, c_int, P, c_int, P]),
@@ -192,13 +189,14 @@ def kernel_launches() -> int:
 _FN = {}
 
 
-def call(name, *args):
-    """Invoke a status-returning entry point on the current CUDA stream and raise on error."""
+def call(name, *args, tail=()):
+    """Invoke a status-returning entry point on the current CUDA stream and raise on error.  `tail`: the arguments that follow
+    the stream in the C signature."""
     global KERNEL_LAUNCHES, ABI_CALLS
     fn = _FN.get(name)
     if fn is None:
         fn = _FN[name] = getattr(lib(), name)
-    rc = fn(*args, stream())
+    rc = fn(*args, stream(), *tail)
     if rc != 0:
         check(rc, name)
     ABI_CALLS += 1

@@ -113,14 +113,10 @@ SIGS = {
     'gcbf_cbf_condition_probe_count': (c_int, [POINTER(FieldDesc), P, P]),
     'gcbf_cbf_condition_probe_fill': (c_int, [POINTER(FieldDesc), P, c_int, c_int, c_int, c_int64, c_int, P, c_int64, P, P, P, P, P, c_int64,
                                               P, P]),
-    'gcbf_linear_fwd_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P]),
-    'gcbf_linear_bwd_data_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
-                                       c_int, c_int, c_int, P]),
-    'gcbf_linear_bwd_weight_t': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, c_int, c_int, c_int, c_int, P]),
-    'gcbf_linear_fwd_tp': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P, c_int]),
-    'gcbf_linear_bwd_data_tp': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
-                                        c_int, c_int, c_int, P, c_int]),
-    'gcbf_linear_bwd_weight_tp': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, c_int, c_int, c_int, c_int, P, c_int]),
+    'gcbf_linear_fwd_h': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, P, c_int, POINTER(H16Desc), P, c_int, c_int, c_int, P, c_int]),
+    'gcbf_linear_bwd_data_h': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, POINTER(H16Desc), P, c_int, c_int, POINTER(H16Desc), P, P,
+                                       c_int, c_int, c_int, P, c_int]),
+    'gcbf_linear_bwd_weight_h': (c_int, [POINTER(H16Desc), POINTER(H16Desc), P, P, c_int, c_int, c_int, c_int, c_int, P, c_int]),
     'gcbf_linear_fwd_emit': (c_int, [P, c_int, P, c_int, P, P, c_int, POINTER(H16Desc), c_int, c_int, c_int, P]),
     'gcbf_launch_count': (c_longlong, [c_int]),
     'gcbf_tc_launch_count': (c_longlong, [c_int, c_int]),

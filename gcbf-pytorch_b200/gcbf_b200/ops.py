@@ -143,12 +143,19 @@ WEIGHT_EPOCH = 0       # bumped whenever a raw kernel rewrites parameters (GCBF.
 class H16:
     """fp16 [hi | lo] companion of an fp32 matrix (same row-major layout, pitch `ld` halves): x * s = hi + lo with the
     per-tensor power-of-two scale s derived from `amax` (device int32 = float bits of max|x|).  One companion serves
-    every GEMM the matrix takes part in (K-major or MN-major operand, csrc/gemm_wgmma_f16.cu)."""
+    every GEMM the matrix takes part in (K-major or MN-major operand, csrc/gemm_wgmma_f16.cu).  Non-zero amax strides: `amax`
+    is an array of per-(128 x 256)-tile maxima instead (what the GEMM epilogues emit)."""
     buf: torch.Tensor
     amax: torch.Tensor
     rows: int
     cols: int
     ld: int
+    amax_row_stride: int = 0
+    amax_col_stride: int = 0
+
+    def desc(self) -> native.H16Desc:
+        """the `gcbf_h16` the tensor-core entry points take (valid while this object keeps the tensors alive)"""
+        return native.H16Desc(ptr(self.buf), ptr(self.amax), self.ld, self.rows, self.cols, self.amax_row_stride, self.amax_col_stride, 0)
 
 
 def use_h(M: int, N: int, K: int) -> bool:
@@ -256,9 +263,8 @@ def linear_fwd_h(xh: H16, wh: H16, b, inv_sigma, act, out=None, out_amax=None):
         out = _empty(M, N, device=xh.buf.device, dtype=torch.float32)
     y, ldy = _mat(out)
     assert y.data_ptr() == out.data_ptr()
-    GEMM_TIMER.run(2.0 * M * N * K, lambda: call('gcbf_linear_fwd_h', ptr(xh.buf), xh.ld, ptr(xh.amax), ptr(wh.buf), wh.ld,
-                                                 ptr(wh.amax), ptr(b), ptr(inv_sigma), ptr(y), ldy, M, N, K, act, ptr(out_amax)), impl=2,
-                   tag=('forward', M, N, K))
+    GEMM_TIMER.run(2.0 * M * N * K, lambda: call('gcbf_linear_fwd_h', xh.desc(), wh.desc(), ptr(b), ptr(inv_sigma), act, ptr(y), ldy, None,
+                                                 ptr(out_amax), M, N, K, tail=(3,)), impl=2, tag=('forward', M, N, K))
     return out
 
 
@@ -273,9 +279,9 @@ def linear_bwd_data_h(dzh: H16, wh: H16, inv_sigma, relu_src, out=None, accumula
     rs, ldr = (None, 0)
     if relu_src is not None:
         rs, ldr = _mat(relu_src)
-    GEMM_TIMER.run(2.0 * M * N * K, lambda: call('gcbf_linear_bwd_data_h', ptr(dzh.buf), dzh.ld, ptr(dzh.amax), ptr(wh.buf), wh.ld,
-                                                 ptr(wh.amax), ptr(inv_sigma), ptr(rs), ldr, ptr(o), ldo, M, N, K,
-                                                 1 if accumulate else 0, ptr(out_amax)), impl=2, tag=('data-grad', M, N, K))
+    GEMM_TIMER.run(2.0 * M * N * K, lambda: call('gcbf_linear_bwd_data_h', dzh.desc(), wh.desc(), ptr(inv_sigma), ptr(rs), ldr, None, ptr(o), ldo,
+                                                 1 if accumulate else 0, None, None, ptr(out_amax), M, N, K, tail=(3,)), impl=2,
+                   tag=('data-grad', M, N, K))
     return out
 
 
@@ -287,9 +293,8 @@ def linear_bwd_weight_h(dzh: H16, xh: H16, inv_sigma, out=None, accumulate=False
         out = _empty(N, K, device=dzh.buf.device, dtype=torch.float32)
     o, ldo = _mat(out)
     assert o.data_ptr() == out.data_ptr() and tuple(o.shape) == (N, K)
-    GEMM_TIMER.run(2.0 * M * N * K, lambda: call('gcbf_linear_bwd_weight_h', ptr(dzh.buf), dzh.ld, ptr(dzh.amax), ptr(xh.buf), xh.ld,
-                                                 ptr(xh.amax), ptr(inv_sigma), ptr(o), ldo, M, N, K, 1 if accumulate else 0), impl=2,
-                   tag=('weight-grad', M, N, K))
+    GEMM_TIMER.run(2.0 * M * N * K, lambda: call('gcbf_linear_bwd_weight_h', dzh.desc(), xh.desc(), ptr(inv_sigma), ptr(o), ldo,
+                                                 1 if accumulate else 0, M, N, K, tail=(3,)), impl=2, tag=('weight-grad', M, N, K))
     return out
 
 

@@ -123,20 +123,38 @@ int gcbf_linear_bwd_weight(const float* dZ, int lddz, const float* X, int ldx, c
 /* ---------------------------------------------------------------------------------------------------
  * K3 on the tensor cores (wgmma + TMA + mbarrier, csrc/gemm_wgmma_f16.cu): the same three products with
  * error-compensated 3xFP16 arithmetic (fp32-grade: 22 significand bits per operand, fp32 accumulation).
- * Operands are "companions": for an fp32 matrix X[rows, cols] the caller provides a device buffer of
- * 2*rows*ld_h halves (ld_h a multiple of 8, 16-byte aligned) that gcbf_split_f16 fills with the planes
- * hi = fp16(X*s), lo = fp16(X*s - hi) in X's own row-major layout; s is the power of two that puts
- * max|X| (device uint32 slot holding its float bits, from gcbf_amax_f32 or a producer's out_amax) into
- * [2^14, 2^15).  One companion serves every product the matrix is in (the tensor core reads it K-major
- * or MN-major), so nothing is transposed or padded:
+ * Operands are "companions", described by a `gcbf_h16`: for an fp32 matrix X[rows, cols] a device buffer of
+ * 2*rows*ld halves (ld a multiple of 8, 16-byte aligned) holding the planes hi = fp16(X*s), lo = fp16(X*s - hi)
+ * in X's own row-major layout; s is the power of two that puts max|X| into [2^14, 2^15).  One companion
+ * serves every product the matrix is in (the tensor core reads it K-major or MN-major), so nothing is
+ * transposed or padded.  The scale is
+ *   per tensor : one device uint32 holding the float bits of max|X| (amax strides 0, 0; from gcbf_amax_f32 or a producer's
+ *                out_amax), planes filled by gcbf_split_f16.  Weight companions are always per-tensor.
+ *   tile-scaled: one word per (128-row, 256-column) tile, amax[rb * amax_row_stride + ct * amax_col_stride] -- the format the
+ *                EPILOGUES emit: every CTA knows the exact maximum of its own 128 x 256 output tile.
  *   fwd_h       : Y  = act(inv_sigma * X W^T + bias)        X[M,K], W[N,K] companions
  *   bwd_data_h  : dX (+)= inv_sigma * dZ W (* relu mask)    dZ[M,N], W[N,K] companions
  *   bwd_weight_h: dW (+)= inv_sigma * dZ^T X                dZ[M,N], X[M,K] companions
- * out_amax (optional, may be NULL): the epilogue atomically maxes |output| into it (zeroed first), which
- * saves the amax pass when the output feeds the next layer's split.  gcbf_split_f16's `colsum`
- * (optional) receives the column sums of the source = the bias gradient when the source is dZ
+ * products: fp16 products per k-slice: 3 = hi*hi + lo*hi + hi*lo (3xFP16), 1 = hi*hi only (fp16 operands, one wgmma per
+ * k-slice; the lo planes are not read).  Any other value is an argument error.
+ * Emission (Yh / dXh, optional, output width > 128, amax strides (ceil(width/256), 1)): a forward / data-grad launch writes its
+ * output directly as a tile-scaled companion, which removes the amax + split passes (and the fp32 round trip through HBM) for
+ * every hidden activation / gradient between two tensor-core layers.  Y / dX may be NULL when only the companion is wanted.
+ * out_amax (optional): the epilogue atomically maxes |output| into it (zeroed first), which saves the amax pass when the
+ * fp32 output feeds the next layer's split.  data-grad extras: the ReLU mask can be read from the hi plane of the layer
+ * output's companion (relu_h instead of relu_src; y > 0 <=> hi > 0), and `colsum` (optional) accumulates (per-row-tile partials
+ * summed in a fixed order) the column sums of the masked output (= the bias gradient of the layer below).
+ * gcbf_split_f16's `colsum` (optional) receives the column sums of the source = the bias gradient when the source is dZ
  * (colsum_accumulate != 0: added to what is there, e.g. the bias's .grad; else overwritten).
  * ------------------------------------------------------------------------------------------------- */
+typedef struct gcbf_h16 {
+  void* buf;                /* hi plane [rows][ld] halves, lo plane at buf + rows * ld halves */
+  void* amax;               /* uint32 float bits of max|x|: per tensor, or per tile */
+  int32_t ld, rows, cols;
+  int32_t amax_row_stride;  /* words between the rows of the tile-maxima array (0: per-tensor) */
+  int32_t amax_col_stride;  /* 1 for a tile-scaled companion, 0 per-tensor */
+  int32_t pad_;
+} gcbf_h16;
 int gcbf_amax_f32(const float* src, int ld, int rows, int cols, void* amax_slot, int accumulate, void* stream);
 int gcbf_split_f16(const float* src, int ld, int rows, int cols, const void* amax_slot, void* dst, int ld_h,
                    float* colsum, int colsum_accumulate, void* stream);
@@ -147,47 +165,13 @@ typedef struct gcbf_split_desc {
 } gcbf_split_desc;
 int gcbf_amax_split_batched(const gcbf_split_desc* descs, int count, void* stream);
 int gcbf_linear_h_supported(int M, int N, int K);
-int gcbf_linear_fwd_h(const void* Xh, int ldxh, const void* x_amax, const void* Wh, int ldwh, const void* w_amax,
-                      const float* bias, const float* inv_sigma, float* Y, int ldy, int M, int N, int K, int act,
-                      void* out_amax, void* stream);
-int gcbf_linear_bwd_data_h(const void* dZh, int lddzh, const void* dz_amax, const void* Wh, int ldwh,
-                           const void* w_amax, const float* inv_sigma, const float* relu_src, int ld_relu,
-                           float* dX, int lddx, int M, int N, int K, int accumulate, void* out_amax, void* stream);
-int gcbf_linear_bwd_weight_h(const void* dZh, int lddzh, const void* dz_amax, const void* Xh, int ldxh,
-                             const void* x_amax, const float* inv_sigma, float* dW, int lddw, int M, int N, int K,
-                             int accumulate, void* stream);
-/* The general form of the three products (ABI v3): operands are `gcbf_h16` descriptors whose scale is either one word per tensor
- * (amax strides 0, what gcbf_split_f16 makes) or one word per (128-row, 256-column) tile of the matrix (amax[rb * amax_row_stride +
- * ct * amax_col_stride]) -- the format the EPILOGUES emit: a forward / data-grad launch can write its output directly as a tile-
- * scaled companion (Yh / dXh, output width > 128), because every CTA knows the exact maximum of its own 128 x 256 tile.  That
- * removes the amax + split passes (and the fp32 round trip through HBM) for every hidden activation / gradient between two
- * tensor-core layers.  Y / dX may be NULL when only the companion is wanted.  data-grad extras: the ReLU mask can be read from
- * the hi plane of the layer output's companion (relu_h; y > 0 <=> hi > 0), and `colsum` (optional) accumulates (per-row-tile partials summed in a fixed order) the
- * column sums of the masked output (= the bias gradient of the layer below).  Weight companions stay per-tensor. */
-typedef struct gcbf_h16 {
-  void* buf;                /* hi plane [rows][ld] halves, lo plane at buf + rows * ld halves */
-  void* amax;               /* uint32 float bits of max|x|: per tensor, or per tile */
-  int32_t ld, rows, cols;
-  int32_t amax_row_stride;  /* words between the rows of the tile-maxima array (0: per-tensor) */
-  int32_t amax_col_stride;  /* 1 for a tile-scaled companion, 0 per-tensor */
-  int32_t pad_;
-} gcbf_h16;
-int gcbf_linear_fwd_t(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
-                      const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream);
-int gcbf_linear_bwd_data_t(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
+int gcbf_linear_fwd_h(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
+                      const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream, int products);
+int gcbf_linear_bwd_data_h(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
                            const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
-                           void* out_amax, int M, int N, int K, void* stream);
-int gcbf_linear_bwd_weight_t(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
-                             int M, int N, int K, void* stream);
-/* The same three products with the number of fp16 products per k-slice: 3 = hi*hi + lo*hi + hi*lo (what the _t functions run),
- * 1 = hi*hi only (fp16 operands, one wgmma per k-slice; the lo planes are not read).  Any other value is an argument error. */
-int gcbf_linear_fwd_tp(const gcbf_h16* X, const gcbf_h16* W, const float* bias, const float* inv_sigma, int act, float* Y, int ldy,
-                       const gcbf_h16* Yh, void* out_amax, int M, int N, int K, void* stream, int products);
-int gcbf_linear_bwd_data_tp(const gcbf_h16* dZ, const gcbf_h16* W, const float* inv_sigma, const float* relu_src, int ld_relu,
-                            const gcbf_h16* relu_h, float* dX, int lddx, int accumulate, const gcbf_h16* dXh, float* colsum,
-                            void* out_amax, int M, int N, int K, void* stream, int products);
-int gcbf_linear_bwd_weight_tp(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
-                              int M, int N, int K, void* stream, int products);
+                           void* out_amax, int M, int N, int K, void* stream, int products);
+int gcbf_linear_bwd_weight_h(const gcbf_h16* dZ, const gcbf_h16* X, const float* inv_sigma, float* dW, int lddw, int accumulate,
+                             int M, int N, int K, void* stream, int products);
 /* wgmma launches issued so far with `products` (3 or 1) fp16 products per k-slice (reset != 0: and set the count to 0): which kernels
  * a pass actually ran, e.g. that every tensor-core layer of a net in fp16 mode took the one-product kernels.  -1 for other values. */
 long long gcbf_tc_launch_count(int products, int reset);

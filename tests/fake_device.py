@@ -312,7 +312,8 @@ def install(monkeypatch, host_lib, jvp_host_lib=None):
     monkeypatch.setattr(torch.cuda, 'Event', _NoEvent)                    # ops.sn_power_iter_batched orders its iterations with events
     monkeypatch.setattr(torch.cuda, 'current_stream', lambda *a, **k: _NoStream())
 
-    def call(name, *args):
+    def call(name, *args, tail=()):
+        args += tuple(tail)                             # (arguments after the stream)
         fn = getattr(fd, name, None)
         if fn is None:
             raise AssertionError(f'fake device: {name} is not emulated (the test reached a kernel outside the MACBF step)')

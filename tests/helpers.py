@@ -5,7 +5,7 @@ import copy
 import torch
 
 import gcbf_oracle as O
-from gcbf_b200 import synth
+from gcbf_b200 import ops, synth
 
 
 def case_inputs(meta):
@@ -30,3 +30,18 @@ def oracle_batch(sb):
 
 def sd_clone(module):
     return {k: v.detach().cpu().clone() for k, v in module.state_dict().items()}
+
+
+def per_tensor(t):
+    """(gcbf_h16 descriptor, the ops.H16 that owns its buffers) of an fp32 device matrix: amax + split kernels, one scale word."""
+    h = ops.split_h(t)
+    return h.desc(), h
+
+
+def tiled_buffers(rows, cols, device='cuda:0'):
+    """(gcbf_h16 descriptor, planes, tile maxima) of a zero-filled tile-scaled companion for an epilogue to write."""
+    ld = (cols + 7) // 8 * 8
+    buf = torch.zeros(2, rows, ld, device=device, dtype=torch.float16)
+    tr, tc = (rows + 127) // 128, (cols + 255) // 256
+    amax = torch.zeros(tr, tc, device=device, dtype=torch.int32)
+    return ops.H16(buf, amax, rows, cols, ld, tc, 1).desc(), buf, amax

@@ -1,4 +1,4 @@
-"""Companions written by the GEMM epilogues (tile-scaled fp16 [hi|lo], gcbf_linear_fwd_t / gcbf_linear_bwd_data_t) and consumed by all
+"""Companions written by the GEMM epilogues (tile-scaled fp16 [hi|lo], gcbf_linear_fwd_h / gcbf_linear_bwd_data_h) and consumed by all
 three products.  The format is pinned bit-for-bit by the CPU model (oracle/fp16x3_model.py::split_tiled): a launch that writes BOTH
 the fp32 output and its companion must produce exactly split_tiled(fp32 output)."""
 import ctypes
@@ -9,6 +9,7 @@ import torch
 
 import fp16x3_model as F16
 from gcbf_b200 import _C, native, ops
+from helpers import per_tensor, tiled_buffers
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0') if torch.cuda.is_available() else None
@@ -18,27 +19,12 @@ def _g(seed):
     return torch.Generator().manual_seed(seed)
 
 
-def per_tensor(t):
-    """(H16Desc, keep-alive) of an fp32 matrix: amax + split kernels, one scale word."""
-    h = ops.split_h(t)
-    d = native.H16Desc(h.buf.data_ptr(), h.amax.data_ptr(), h.ld, h.rows, h.cols, 0, 0, 0)
-    return d, h
-
-
-def tiled_buffers(rows, cols):
-    ld = (cols + 7) // 8 * 8
-    buf = torch.zeros(2, rows, ld, device=DEV, dtype=torch.float16)
-    tr, tc = (rows + 127) // 128, (cols + 255) // 256
-    amax = torch.zeros(tr, tc, device=DEV, dtype=torch.int32)
-    return native.H16Desc(buf.data_ptr(), amax.data_ptr(), ld, rows, cols, tc, 1, 0), buf, amax
-
-
 def fwd(X, W, b, alpha, act, M, N, K, want_f32=True, emit=True):
     y = torch.empty(M, N, device=DEV) if want_f32 else None
     yd, ybuf, yamax = tiled_buffers(M, N)
-    rc = native.fn('gcbf_linear_fwd_t')(ctypes.byref(X), ctypes.byref(W), _C.ptr(b), _C.ptr(alpha), act, _C.ptr(y), N,
-                                        ctypes.byref(yd) if emit else None, None, M, N, K, _C.stream())
-    native.check(rc, 'gcbf_linear_fwd_t')
+    rc = native.fn('gcbf_linear_fwd_h')(ctypes.byref(X), ctypes.byref(W), _C.ptr(b), _C.ptr(alpha), act, _C.ptr(y), N,
+                                        ctypes.byref(yd) if emit else None, None, M, N, K, _C.stream(), 3)
+    native.check(rc, 'gcbf_linear_fwd_h')
     return y, (yd, ybuf, yamax)
 
 
@@ -80,8 +66,8 @@ def test_tile_scaled_operands_in_all_three_products(M, N, K):
     y1, (y1d, y1buf, y1amax) = fwd(X, W1h, zero_b, None, ops.ACT_RELU, M, K, K)                       # [M, K] hidden activation, emitted
     # forward through layer 2 from the emitted companion
     y2 = torch.empty(M, N, device=DEV)
-    native.check(native.fn('gcbf_linear_fwd_t')(ctypes.byref(y1d), ctypes.byref(W2h), None, None, ops.ACT_NONE, _C.ptr(y2), N, None, None, M, N, K,
-                                                _C.stream()), 'fwd2')
+    native.check(native.fn('gcbf_linear_fwd_h')(ctypes.byref(y1d), ctypes.byref(W2h), None, None, ops.ACT_NONE, _C.ptr(y2), N, None, None, M, N, K,
+                                                _C.stream(), 3), 'fwd2')
     y1_64 = y1.double()
     e = lambda a, r: ((a.double() - r).abs().max() / r.abs().max()).item()
     assert e(y2, y1_64 @ W2d.double().t()) < 1e-5
@@ -90,8 +76,8 @@ def test_tile_scaled_operands_in_all_three_products(M, N, K):
     dx = torch.empty(M, K, device=DEV)
     dxd, dxbuf, dxamax = tiled_buffers(M, K)
     colsum = torch.zeros(K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_data_t')(ctypes.byref(DZ), ctypes.byref(W2h), None, None, 0, ctypes.byref(y1d), _C.ptr(dx), K, 0,
-                                                     ctypes.byref(dxd), _C.ptr(colsum), None, M, N, K, _C.stream()), 'dgrad')
+    native.check(native.fn('gcbf_linear_bwd_data_h')(ctypes.byref(DZ), ctypes.byref(W2h), None, None, 0, ctypes.byref(y1d), _C.ptr(dx), K, 0,
+                                                     ctypes.byref(dxd), _C.ptr(colsum), None, M, N, K, _C.stream(), 3), 'dgrad')
     torch.cuda.synchronize()
     want_dx = (dzd.double() @ W2d.double()) * (y1 > 0)
     assert e(dx, want_dx) < 1e-5
@@ -101,16 +87,16 @@ def test_tile_scaled_operands_in_all_three_products(M, N, K):
     assert ((colsum.double() - dx.double().sum(0)).abs().max() / dx.double().sum(0).abs().max()).item() < 1e-5
     # mask from the fp32 activation gives the same result
     dx2 = torch.empty(M, K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_data_t')(ctypes.byref(DZ), ctypes.byref(W2h), None, _C.ptr(y1), K, None, _C.ptr(dx2), K, 0, None, None,
-                                                     None, M, N, K, _C.stream()), 'dgrad2')
+    native.check(native.fn('gcbf_linear_bwd_data_h')(ctypes.byref(DZ), ctypes.byref(W2h), None, _C.ptr(y1), K, None, _C.ptr(dx2), K, 0, None, None,
+                                                     None, M, N, K, _C.stream(), 3), 'dgrad2')
     assert torch.equal(dx2, dx)
     # weight-grad of layer 1 (dW1 = dx^T x... here: operands dx (emitted, tile-scaled) and y1 (emitted, tile-scaled)): dW = dx^T y1
     dW = torch.empty(K, K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_weight_t')(ctypes.byref(dxd), ctypes.byref(y1d), None, _C.ptr(dW), K, 0, M, K, K, _C.stream()), 'wgrad')
+    native.check(native.fn('gcbf_linear_bwd_weight_h')(ctypes.byref(dxd), ctypes.byref(y1d), None, _C.ptr(dW), K, 0, M, K, K, _C.stream(), 3), 'wgrad')
     assert e(dW, dx.double().t() @ y1_64) < 1e-5
     # and mixed: per-tensor dZ with the tile-scaled activation (what the first backward layer of a chain sees)
     dW2 = torch.empty(N, K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_weight_t')(ctypes.byref(DZ), ctypes.byref(y1d), None, _C.ptr(dW2), K, 0, M, N, K, _C.stream()), 'wgrad2')
+    native.check(native.fn('gcbf_linear_bwd_weight_h')(ctypes.byref(DZ), ctypes.byref(y1d), None, _C.ptr(dW2), K, 0, M, N, K, _C.stream(), 3), 'wgrad2')
     assert e(dW2, dzd.double().t() @ y1_64) < 1e-5
 
 
@@ -130,8 +116,8 @@ def test_cpu_model_of_tile_scaled_products_matches_the_kernel():
     assert torch.equal(y, xd.abs())                                   # exact: small integers
     Wh, k2 = per_tensor(Wd)
     out = torch.empty(M, N, device=DEV)
-    native.check(native.fn('gcbf_linear_fwd_t')(ctypes.byref(yd), ctypes.byref(Wh), None, None, ops.ACT_NONE, _C.ptr(out), N, None, None, M, N, K,
-                                                _C.stream()), 'fwd')
+    native.check(native.fn('gcbf_linear_fwd_h')(ctypes.byref(yd), ctypes.byref(Wh), None, None, ops.ACT_NONE, _C.ptr(out), N, None, None, M, N, K,
+                                                _C.stream(), 3), 'fwd')
     want = F16.gemm_tiled_a(x.abs(), W)
     assert torch.equal(out.cpu(), want)
 

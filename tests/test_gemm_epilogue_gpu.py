@@ -1,4 +1,4 @@
-"""Data-grad epilogue of the wgmma GEMM (gcbf_linear_bwd_data_tp) at the edges of the work it does after the mainloop: the ReLU mask
+"""Data-grad epilogue of the wgmma GEMM (gcbf_linear_bwd_data_h) at the edges of the work it does after the mainloop: the ReLU mask
 (loaded before the parked tile is touched, from either source), tile maxima, the emitted companion and the column sums.
 
 Shapes put that work on its edges: contractions of one to eight k-blocks (half 1 of a 256-wide tile shorter than any slice of the
@@ -14,23 +14,11 @@ import pytest
 import torch
 
 import fp16x3_model as F16
-from gcbf_b200 import _C, native, ops
+from gcbf_b200 import _C, native
+from helpers import per_tensor, tiled_buffers
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0') if torch.cuda.is_available() else None
-
-
-def per_tensor(t):
-    h = ops.split_h(t)
-    return native.H16Desc(h.buf.data_ptr(), h.amax.data_ptr(), h.ld, h.rows, h.cols, 0, 0, 0), h
-
-
-def tiled_buffers(rows, cols):
-    ld = (cols + 7) // 8 * 8
-    buf = torch.zeros(2, rows, ld, device=DEV, dtype=torch.float16)
-    tr, tc = (rows + 127) // 128, (cols + 255) // 256
-    amax = torch.zeros(tr, tc, device=DEV, dtype=torch.int32)
-    return native.H16Desc(buf.data_ptr(), amax.data_ptr(), ld, rows, cols, tc, 1, 0), buf, amax
 
 
 def colsum_in_kernel_order(x):
@@ -60,11 +48,11 @@ def dgrad(products, DZ, W, alpha, mask_src, mask_h, M, N, K):
     dx = torch.full((M, K), float('nan'), device=DEV)
     dxd, dxbuf, dxamax = tiled_buffers(M, K)
     colsum = torch.zeros(K, device=DEV)
-    rc = native.fn('gcbf_linear_bwd_data_tp')(ctypes.byref(DZ), ctypes.byref(W), _C.ptr(alpha),
+    rc = native.fn('gcbf_linear_bwd_data_h')(ctypes.byref(DZ), ctypes.byref(W), _C.ptr(alpha),
                                               _C.ptr(mask_src[0]) if mask_src else None, mask_src[1] if mask_src else 0,
                                               ctypes.byref(mask_h) if mask_h is not None else None, _C.ptr(dx), K, 0,
                                               ctypes.byref(dxd), _C.ptr(colsum), None, M, N, K, _C.stream(), products)
-    native.check(rc, 'gcbf_linear_bwd_data_tp')
+    native.check(rc, 'gcbf_linear_bwd_data_h')
     torch.cuda.synchronize()
     return dx.cpu(), dxbuf.cpu(), dxamax.cpu(), colsum.cpu()
 

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f'{name} declared in include/gcbf_b200.h but not exported'
     assert sorted(_C.EXPORTED_SYMBOLS) == declared, set(_C.EXPORTED_SYMBOLS) ^ set(declared)
-    assert _C.lib().gcbf_abi_version() == 5
+    assert _C.lib().gcbf_abi_version() == 6
 
 
 def test_env_cfg_struct_layout():
@@ -363,14 +363,20 @@ def test_c_abi_rejects_bad_arguments_before_touching_the_gpu():
     assert lib.gcbf_split_f16(ok_ptr, 64, 4, 64, ok_ptr, ok_ptr, 60, None, 0, None) == -1 and ('pitch' in err() or 'bad arguments' in err())
     assert lib.gcbf_split_f16(ok_ptr, 32, 4, 64, ok_ptr, ok_ptr, 64, None, 0, None) == -1          # ld < cols
     assert lib.gcbf_amax_f32(ok_ptr, 8, 4, 8, None, 0, None) == -1                                  # no amax slot
-    # GEMM entry points: missing amax words, output pitch smaller than the row, misaligned companions
-    args = dict(Xh=ok_ptr, ldx=64, xa=ok_ptr, Wh=ok_ptr, ldw=64, wa=ok_ptr)
-    assert lib.gcbf_linear_fwd_h(args['Xh'], 64, None, args['Wh'], 64, ok_ptr, None, None, ok_ptr, 256, 512, 256, 64, 0, None, None) == -1
-    assert lib.gcbf_linear_fwd_h(args['Xh'], 64, ok_ptr, args['Wh'], 64, ok_ptr, None, None, ok_ptr, 100, 512, 256, 64, 0, None, None) == -1
-    assert lib.gcbf_linear_fwd_h(odd_ptr, 64, ok_ptr, args['Wh'], 64, ok_ptr, None, None, ok_ptr, 256, 512, 256, 64, 0, None, None) == -1
-    assert 'gcbf_linear_fwd_' in err()          # (the per-tensor entry points forward to the general gcbf_linear_fwd_t)
-    assert lib.gcbf_linear_bwd_data_h(ok_ptr, 256, ok_ptr, ok_ptr, 64, ok_ptr, None, ok_ptr, 32, ok_ptr, 64, 512, 256, 64, 0, None, None) == -1   # ld_relu < K
-    assert lib.gcbf_linear_bwd_weight_h(ok_ptr, 256, ok_ptr, ok_ptr, 62, ok_ptr, None, ok_ptr, 64, 512, 256, 64, 0, None) == -1    # pitch not a multiple of 8
+    # GEMM entry points: missing amax word, output pitch smaller than the row, misaligned companion, descriptor of another shape
+    H, (M, N, K) = native.H16Desc, (512, 256, 64)
+    W, dZ = H(ok_ptr, ok_ptr, 64, N, K, 0, 0, 0), H(ok_ptr, ok_ptr, 256, M, N, 0, 0, 0)
+
+    def fwd(buf=ok_ptr, amax=ok_ptr, cols=K, ldy=256):
+        return lib.gcbf_linear_fwd_h(H(buf, amax, 64, M, cols, 0, 0, 0), W, None, None, 0, ok_ptr, ldy, None, None, M, N, K, None, 3)
+    assert fwd(amax=None) == -1 and err().startswith('gcbf_linear_fwd_h X:')
+    assert fwd(ldy=100) == -1 and err().startswith('gcbf_linear_fwd_h: bad arguments')
+    assert fwd(buf=odd_ptr) == -1 and err().startswith('gcbf_linear_fwd_h X:') and 'aligned' in err()
+    assert fwd(cols=K - 8) == -1 and err().startswith('gcbf_linear_fwd_h X: companion descriptor')   # X is not [M x K]
+    assert lib.gcbf_linear_bwd_data_h(dZ, W, None, ok_ptr, 32, None, ok_ptr, 64, 0, None, None, None, M, N, K, None, 3) == -1   # ld_relu < K
+    assert err().startswith('gcbf_linear_bwd_data_h: ld_relu')
+    assert lib.gcbf_linear_bwd_weight_h(dZ, H(ok_ptr, ok_ptr, 68, M, K, 0, 0, 0), None, ok_ptr, 64, 0, M, N, K, None, 3) == -1   # pitch not a multiple of 8
+    assert err().startswith('gcbf_linear_bwd_weight_h X:') and 'pitch' in err()
     assert lib.gcbf_amax_split_batched(None, 3, None) == -1
     assert lib.gcbf_sn_power_iter_batched(None, 1, ok_ptr, 0, None) == -1
     # the fp32 entry points keep their "tensor-core path has its own entry point" answer for impl = 2

@@ -80,7 +80,7 @@ def _tc_kch(product):
 
 
 def wgmma_wgrad_splits(M, N, K):
-    """Contraction splits of the wgmma weight-grad (gcbf_linear_bwd_weight_t, then th::launch's chunk rounding)."""
+    """Contraction splits of the wgmma weight-grad (gcbf_linear_bwd_weight_h, then th::launch's chunk rounding)."""
     bn = 256 if K > 128 else 128
     tiles = _cdiv(N, 128) * _cdiv(K, bn)
     splits = max(1, min(_cdiv(M, 256), NUM_SMS // tiles)) if tiles < NUM_SMS else 1

@@ -97,11 +97,12 @@ def test_tc_products_sits_where_pad_was():
     assert native.NetDesc().tc_products == 0                # zero-initialised descriptors keep the 3xFP16 default
 
 
-def test_tp_entry_points_are_declared_with_their_t_signature_plus_products():
+def test_tensor_core_entry_points_take_products_after_the_stream():
     for name in ('gcbf_linear_fwd', 'gcbf_linear_bwd_data', 'gcbf_linear_bwd_weight'):
-        rt, args = native.SIGS[name + '_t']
-        rtp, argsp = native.SIGS[name + '_tp']
-        assert rtp is rt and argsp == args + [ctypes.c_int]
+        rt, args = native.SIGS[name + '_h']
+        assert rt is ctypes.c_int and args[-2:] == [native.P, ctypes.c_int]
+        assert args[:2] == [ctypes.POINTER(native.H16Desc)] * 2
+        assert name + '_t' not in native.SIGS and name + '_tp' not in native.SIGS      # one generation of the three products
 
 
 # ---- the rounding model ---------------------------------------------------------------------------------------------------------

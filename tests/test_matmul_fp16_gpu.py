@@ -1,4 +1,4 @@
-"""The one-product tensor-core mode (gcbf_linear_*_tp with products = 1; GCBF.params['matmul'] = 'fp16') on the GPU.
+"""The one-product tensor-core mode (gcbf_linear_*_h with products = 1; GCBF.params['matmul'] = 'fp16') on the GPU.
 
   * per product: every product kind, both tile widths, ragged shapes, split-K, per-tensor and tile-scaled operands, strided outputs
     and accumulation, each element within the bound derived in tests/matmul_fp16_model.py against float64 of the fp32 operands;
@@ -18,7 +18,7 @@ import fp16x3_model as F16
 import gcbf_oracle as O
 import matmul_fp16_model as F1
 from gcbf_b200 import _C, native, ops, synth
-from helpers import oracle_batch, product_batch, sd_clone, seeded_algo
+from helpers import oracle_batch, per_tensor, product_batch, sd_clone, seeded_algo, tiled_buffers
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda:0') if torch.cuda.is_available() else None
@@ -27,19 +27,6 @@ L_MAX = 256          # the longest promotion chunk (data-grad with a per-tensor 
 
 def _g(seed):
     return torch.Generator().manual_seed(seed)
-
-
-def per_tensor(t):
-    h = ops.split_h(t)
-    return native.H16Desc(h.buf.data_ptr(), h.amax.data_ptr(), h.ld, h.rows, h.cols, 0, 0, 0), h
-
-
-def tiled_buffers(rows, cols):
-    ld = (cols + 7) // 8 * 8
-    buf = torch.zeros(2, rows, ld, device=DEV, dtype=torch.float16)
-    tr, tc = (rows + 127) // 128, (cols + 255) // 256
-    amax = torch.zeros(tr, tc, device=DEV, dtype=torch.int32)
-    return native.H16Desc(buf.data_ptr(), amax.data_ptr(), ld, rows, cols, tc, 1, 0), buf, amax
 
 
 def strided(rows, cols, extra=5):
@@ -65,10 +52,10 @@ def _conservative(Kc):
     return L_MAX, kb, kb
 
 
-def fwd_tp(X, W, b, alpha, act, y, ldy, Yh, M, N, K, products=1):
-    native.check(native.fn('gcbf_linear_fwd_tp')(ctypes.byref(X), ctypes.byref(W), _C.ptr(b), _C.ptr(alpha), act, _C.ptr(y), ldy,
+def fwd_h(X, W, b, alpha, act, y, ldy, Yh, M, N, K, products=1):
+    native.check(native.fn('gcbf_linear_fwd_h')(ctypes.byref(X), ctypes.byref(W), _C.ptr(b), _C.ptr(alpha), act, _C.ptr(y), ldy,
                                                  ctypes.byref(Yh) if Yh is not None else None, None, M, N, K, _C.stream(), products),
-                 'gcbf_linear_fwd_tp')
+                 'gcbf_linear_fwd_h')
 
 
 # ---- per-product bound ------------------------------------------------------------------------------------------------------------
@@ -84,7 +71,7 @@ def test_forward_within_bound(M, N, K, bias):
     X, k0 = per_tensor(xd)
     Wh, k1 = per_tensor(Wd)
     buf, y, ldy = strided(M, N)
-    fwd_tp(X, Wh, bd, alpha, ops.ACT_NONE, buf, ldy, None, M, N, K)
+    fwd_h(X, Wh, bd, alpha, ops.ACT_NONE, buf, ldy, None, M, N, K)
     torch.cuda.synchronize()
     a, bm = x.numpy(), W.t().contiguous().numpy()
     ref = 0.7 * (a.astype(np.float64) @ bm.astype(np.float64)) + (b.double().numpy()[None, :] if bias else 0.0)
@@ -109,8 +96,8 @@ def test_data_grad_within_bound(M, N, K, accumulate, mask):
     buf, dx, ld = strided(M, K)
     if accumulate:
         dx.copy_(prev.to(DEV))
-    native.check(native.fn('gcbf_linear_bwd_data_tp')(ctypes.byref(DZ), ctypes.byref(Wh), None, _C.ptr(srcd) if mask else None, K, None,
-                                                      _C.ptr(buf), ld, accumulate, None, None, None, M, N, K, _C.stream(), 1), 'dgrad_tp')
+    native.check(native.fn('gcbf_linear_bwd_data_h')(ctypes.byref(DZ), ctypes.byref(Wh), None, _C.ptr(srcd) if mask else None, K, None,
+                                                      _C.ptr(buf), ld, accumulate, None, None, None, M, N, K, _C.stream(), 1), 'dgrad')
     torch.cuda.synchronize()
     a, bm = dz.numpy(), W.numpy()
     m = (src.numpy() > 0) if mask else np.ones((M, K), bool)
@@ -134,8 +121,8 @@ def test_weight_grad_within_bound(M, N, K, accumulate):
     buf, dW, ld = strided(N, K)
     if accumulate:
         dW.copy_(prev.to(DEV))
-    native.check(native.fn('gcbf_linear_bwd_weight_tp')(ctypes.byref(DZ), ctypes.byref(X), None, _C.ptr(buf), ld, accumulate, M, N, K,
-                                                        _C.stream(), 1), 'wgrad_tp')
+    native.check(native.fn('gcbf_linear_bwd_weight_h')(ctypes.byref(DZ), ctypes.byref(X), None, _C.ptr(buf), ld, accumulate, M, N, K,
+                                                        _C.stream(), 1), 'wgrad')
     torch.cuda.synchronize()
     a, bm = dz.t().contiguous().numpy(), x.numpy()
     ref = a.astype(np.float64) @ bm.astype(np.float64) + (prev.double().numpy() if accumulate else 0.0)
@@ -162,7 +149,7 @@ def test_emission_and_tile_scaled_operands(M, N, K):
     W2h, k2 = per_tensor(W2d)
     y1 = torch.empty(M, K, device=DEV)
     y1d, y1buf, y1amax = tiled_buffers(M, K)
-    fwd_tp(X, W1h, torch.zeros(K, device=DEV), None, ops.ACT_RELU, y1, K, y1d, M, K, K)
+    fwd_h(X, W1h, torch.zeros(K, device=DEV), None, ops.ACT_RELU, y1, K, y1d, M, K, K)
     torch.cuda.synchronize()
     hi, lo, amax = F16.split_tiled(y1.cpu())
     assert torch.equal(y1amax.view(torch.float32).cpu(), amax)
@@ -171,7 +158,7 @@ def test_emission_and_tile_scaled_operands(M, N, K):
     s1 = F1.tile_scales(a1)
     # forward from the emitted (tile-scaled) companion
     y2 = torch.empty(M, N, device=DEV)
-    fwd_tp(y1d, W2h, None, None, ops.ACT_NONE, y2, N, None, M, N, K)
+    fwd_h(y1d, W2h, None, None, ops.ACT_NONE, y2, N, None, M, N, K)
     w2t = W2.t().contiguous().numpy()
     L, n, s = _conservative(K)
     _assert_bound(y2, a1.astype(np.float64) @ w2t.astype(np.float64), F1.bound(a1, w2t, s1, F1.tensor_scales(w2t), L, n, s), 'forward (tiled A)')
@@ -180,8 +167,8 @@ def test_emission_and_tile_scaled_operands(M, N, K):
     dx = torch.empty(M, K, device=DEV)
     dxd, dxbuf, dxamax = tiled_buffers(M, K)
     colsum = torch.zeros(K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_data_tp')(ctypes.byref(DZ), ctypes.byref(W2h), None, None, 0, ctypes.byref(y1d), _C.ptr(dx), K, 0,
-                                                      ctypes.byref(dxd), _C.ptr(colsum), None, M, N, K, _C.stream(), 1), 'dgrad_tp')
+    native.check(native.fn('gcbf_linear_bwd_data_h')(ctypes.byref(DZ), ctypes.byref(W2h), None, None, 0, ctypes.byref(y1d), _C.ptr(dx), K, 0,
+                                                      ctypes.byref(dxd), _C.ptr(colsum), None, M, N, K, _C.stream(), 1), 'dgrad')
     torch.cuda.synchronize()
     mask = a1 > 0
     a, bm = dz.numpy(), W2.numpy()
@@ -196,11 +183,11 @@ def test_emission_and_tile_scaled_operands(M, N, K):
     assert np.all(np.abs(_np(colsum) - dx64.sum(0)) <= cs_bound)
     # weight-grads: both operands tile-scaled (dx, y1), and a per-tensor dZ with the tile-scaled y1
     dW = torch.empty(K, K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_weight_tp')(ctypes.byref(dxd), ctypes.byref(y1d), None, _C.ptr(dW), K, 0, M, K, K, _C.stream(), 1),
-                 'wgrad_tp')
+    native.check(native.fn('gcbf_linear_bwd_weight_h')(ctypes.byref(dxd), ctypes.byref(y1d), None, _C.ptr(dW), K, 0, M, K, K, _C.stream(), 1),
+                 'wgrad')
     dW2 = torch.empty(N, K, device=DEV)
-    native.check(native.fn('gcbf_linear_bwd_weight_tp')(ctypes.byref(DZ), ctypes.byref(y1d), None, _C.ptr(dW2), K, 0, M, N, K, _C.stream(), 1),
-                 'wgrad2_tp')
+    native.check(native.fn('gcbf_linear_bwd_weight_h')(ctypes.byref(DZ), ctypes.byref(y1d), None, _C.ptr(dW2), K, 0, M, N, K, _C.stream(), 1),
+                 'wgrad2')
     torch.cuda.synchronize()
     dxf = dx.cpu().numpy()
     L, n, s = _conservative(M)
@@ -217,14 +204,12 @@ def test_products_argument_is_checked():
     W, k1 = per_tensor(torch.randn(128, 128, device=DEV))
     y = torch.empty(256, 128, device=DEV)
     for bad in (0, 2, 4, -1):
-        rc = native.fn('gcbf_linear_fwd_tp')(ctypes.byref(X), ctypes.byref(W), None, None, 0, _C.ptr(y), 128, None, None, 256, 128, 128,
+        rc = native.fn('gcbf_linear_fwd_h')(ctypes.byref(X), ctypes.byref(W), None, None, 0, _C.ptr(y), 128, None, None, 256, 128, 128,
                                             _C.stream(), bad)
         assert rc != 0
-    # products = 3 is the _t function, bit for bit
-    y3 = torch.empty_like(y)
-    fwd_tp(X, W, None, None, 0, y, 128, None, 256, 128, 128, products=3)
-    native.check(native.fn('gcbf_linear_fwd_t')(ctypes.byref(X), ctypes.byref(W), None, None, 0, _C.ptr(y3), 128, None, None, 256, 128, 128,
-                                                _C.stream()), 'fwd_t')
+    # products = 3 is the default (3xFP16) path, bit for bit
+    fwd_h(X, W, None, None, 0, y, 128, None, 256, 128, 128, products=3)
+    y3 = ops.linear_fwd_h(k0, k1, None, None, 0)
     assert torch.equal(y, y3)
 
 

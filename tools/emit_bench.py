@@ -23,7 +23,7 @@ def tiled(rows, cols):
     buf = torch.zeros(2, rows, ld, device=dev, dtype=torch.float16)
     tc = (cols + 255) // 256
     amax = torch.zeros((rows + 127) // 128, tc, device=dev, dtype=torch.int32)
-    return native.H16Desc(buf.data_ptr(), amax.data_ptr(), ld, rows, cols, tc, 1, 0), (buf, amax)
+    return ops.H16(buf, amax, rows, cols, ld, tc, 1).desc(), (buf, amax)
 
 
 print('GCBF_EPI_STORE =', os.environ.get('GCBF_EPI_STORE', 'tma'), ' GCBF_TC_KCH =', os.environ.get('GCBF_TC_KCH', '4'))
@@ -31,25 +31,23 @@ for M in [int(a) for a in sys.argv[1:]] or [24196, 206139]:
     N = K = 2048
     x = torch.randn(M, K, device=dev); W = torch.randn(N, K, device=dev) / 45; b = torch.zeros(N, device=dev); dz = torch.randn(M, N, device=dev)
     xh, wh, dzh = ops.split_h(x), ops.split_h(W), ops.split_h(dz)
-    X = native.H16Desc(xh.buf.data_ptr(), xh.amax.data_ptr(), xh.ld, M, K, 0, 0, 0)
-    Wd = native.H16Desc(wh.buf.data_ptr(), wh.amax.data_ptr(), wh.ld, N, K, 0, 0, 0)
-    DZ = native.H16Desc(dzh.buf.data_ptr(), dzh.amax.data_ptr(), dzh.ld, M, N, 0, 0, 0)
+    X, Wd, DZ = xh.desc(), wh.desc(), dzh.desc()
     y = torch.empty(M, N, device=dev)
     yd, keep = tiled(M, N)
     colsum = torch.zeros(K, device=dev)
     fl = 2.0 * M * N * K
-    F, D = native.fn('gcbf_linear_fwd_t'), native.fn('gcbf_linear_bwd_data_t')
+    F, D = native.fn('gcbf_linear_fwd_h'), native.fn('gcbf_linear_bwd_data_h')
     st = _C.stream()
     modes = {
-        'fwd fp32 out': lambda: F(ctypes.byref(X), ctypes.byref(Wd), b.data_ptr(), None, 1, y.data_ptr(), N, None, None, M, N, K, st),
-        'fwd companion out': lambda: F(ctypes.byref(X), ctypes.byref(Wd), b.data_ptr(), None, 1, None, N, ctypes.byref(yd), None, M, N, K, st),
-        'fwd both': lambda: F(ctypes.byref(X), ctypes.byref(Wd), b.data_ptr(), None, 1, y.data_ptr(), N, ctypes.byref(yd), None, M, N, K, st),
-        'fwd from tile-scaled A': lambda: F(ctypes.byref(yd), ctypes.byref(Wd), b.data_ptr(), None, 1, y.data_ptr(), N, None, None, M, N, K, st),
-        'dgrad fp32 out, fp32 mask': lambda: D(ctypes.byref(DZ), ctypes.byref(Wd), None, x.data_ptr(), K, None, y.data_ptr(), K, 0, None, None, None, M, N, K, st),
+        'fwd fp32 out': lambda: F(ctypes.byref(X), ctypes.byref(Wd), b.data_ptr(), None, 1, y.data_ptr(), N, None, None, M, N, K, st, 3),
+        'fwd companion out': lambda: F(ctypes.byref(X), ctypes.byref(Wd), b.data_ptr(), None, 1, None, N, ctypes.byref(yd), None, M, N, K, st, 3),
+        'fwd both': lambda: F(ctypes.byref(X), ctypes.byref(Wd), b.data_ptr(), None, 1, y.data_ptr(), N, ctypes.byref(yd), None, M, N, K, st, 3),
+        'fwd from tile-scaled A': lambda: F(ctypes.byref(yd), ctypes.byref(Wd), b.data_ptr(), None, 1, y.data_ptr(), N, None, None, M, N, K, st, 3),
+        'dgrad fp32 out, fp32 mask': lambda: D(ctypes.byref(DZ), ctypes.byref(Wd), None, x.data_ptr(), K, None, y.data_ptr(), K, 0, None, None, None, M, N, K, st, 3),
         'dgrad companion out, hi mask, colsum': lambda: D(ctypes.byref(DZ), ctypes.byref(Wd), None, None, 0, ctypes.byref(X), None, K, 0, ctypes.byref(yd),
-                                                          colsum.data_ptr(), None, M, N, K, st),
+                                                          colsum.data_ptr(), None, M, N, K, st, 3),
         'dgrad companion out, hi mask': lambda: D(ctypes.byref(DZ), ctypes.byref(Wd), None, None, 0, ctypes.byref(X), None, K, 0, ctypes.byref(yd), None, None,
-                                                  M, N, K, st),
+                                                  M, N, K, st, 3),
     }
     for name, fn in modes.items():
         rc = fn()

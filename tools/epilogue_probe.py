@@ -56,15 +56,11 @@ def step_launches(cfg, dev):
     return E, A, shapes
 
 
-def desc(h):
-    return native.H16Desc(h.buf.data_ptr(), h.amax.data_ptr(), h.ld, h.rows, h.cols, 0, 0, 0)
-
-
 def tiled(rows, cols, dev):
     ld = (cols + 7) // 8 * 8
     buf = torch.zeros(2, rows, ld, device=dev, dtype=torch.float16)
     amax = torch.zeros((rows + 127) // 128, (cols + 255) // 256, device=dev, dtype=torch.int32)
-    return native.H16Desc(buf.data_ptr(), amax.data_ptr(), ld, rows, cols, amax.shape[1], 1, 0), (buf, amax)
+    return ops.H16(buf, amax, rows, cols, ld, amax.shape[1], 1).desc(), (buf, amax)
 
 
 def timeit(fn, n):
@@ -85,13 +81,13 @@ def probe(kind, M, N, K, tc_shapes, dev, reps):
     g = torch.Generator(device=dev).manual_seed(M + N + K)
     W = torch.randn(N, K, device=dev, generator=g) / K ** 0.5
     wh = ops.split_h(W)
-    Wd = desc(wh)
+    Wd = wh.desc()
     isg = torch.full((1,), 0.9, device=dev)
     st = _C.stream()
     if kind == 0:
-        f = native.fn('gcbf_linear_fwd_t')
+        f = native.fn('gcbf_linear_fwd_h')
         xh = ops.split_h(torch.randn(M, K, device=dev, generator=g))
-        X = desc(xh)
+        X = xh.desc()
         b = torch.randn(N, device=dev, generator=g) * 0.1
         y = torch.empty(M, N, device=dev)
         # a hidden layer of the step feeds a tensor-core layer: companion only; the last layer of a net writes fp32
@@ -99,14 +95,14 @@ def probe(kind, M, N, K, tc_shapes, dev, reps):
         Yh, keep = tiled(M, N, dev) if hidden else (None, None)
         opts = 'bias, alpha, ReLU, companion' if hidden else 'bias, alpha, fp32'
         epi = lambda: native.check(f(ctypes.byref(X), ctypes.byref(Wd), _C.ptr(b), _C.ptr(isg), ops.ACT_RELU if hidden else 0,
-                                     None if hidden else _C.ptr(y), N, ctypes.byref(Yh) if hidden else None, None, M, N, K, st), 'fwd')
-        plain = lambda: native.check(f(ctypes.byref(X), ctypes.byref(Wd), None, None, 0, _C.ptr(y), N, None, None, M, N, K, st), 'fwd')
+                                     None if hidden else _C.ptr(y), N, ctypes.byref(Yh) if hidden else None, None, M, N, K, st, 3), 'fwd')
+        plain = lambda: native.check(f(ctypes.byref(X), ctypes.byref(Wd), None, None, 0, _C.ptr(y), N, None, None, M, N, K, st, 3), 'fwd')
     else:
-        f = native.fn('gcbf_linear_bwd_data_t')
+        f = native.fn('gcbf_linear_bwd_data_h')
         dzh = ops.split_h(torch.randn(M, N, device=dev, generator=g) * 1e-3)
-        DZ = desc(dzh)
+        DZ = dzh.desc()
         maskh = ops.split_h(torch.randn(M, K, device=dev, generator=g))
-        MK = desc(maskh)
+        MK = maskh.desc()
         dx = torch.empty(M, K, device=dev)
         colsum = torch.zeros(K, device=dev)
         # the layer below (K outputs) is a hidden layer; it runs on the tensor cores iff the step has a forward [M, K] launch
@@ -117,9 +113,9 @@ def probe(kind, M, N, K, tc_shapes, dev, reps):
         opts = ', '.join(['alpha'] + (['hi-plane mask'] if mask else []) + (['companion, column sums'] if emit else ['fp32']))
         epi = lambda: native.check(f(ctypes.byref(DZ), ctypes.byref(Wd), _C.ptr(isg), None, 0, ctypes.byref(MK) if mask else None,
                                      None if emit else _C.ptr(dx), K, 0, ctypes.byref(dXh) if emit else None,
-                                     _C.ptr(colsum) if emit else None, None, M, N, K, st), 'dgrad')
+                                     _C.ptr(colsum) if emit else None, None, M, N, K, st, 3), 'dgrad')
         plain = lambda: native.check(f(ctypes.byref(DZ), ctypes.byref(Wd), None, None, 0, None, _C.ptr(dx), K, 0, None, None, None,
-                                       M, N, K, st), 'dgrad')
+                                       M, N, K, st, 3), 'dgrad')
     t_e, t_p = timeit(epi, reps), timeit(plain, reps)
     t_e2, t_p2 = timeit(epi, reps), timeit(plain, reps)     # alternated twice: the lower of each pair is kept
     return min(t_e, t_e2), min(t_p, t_p2), opts

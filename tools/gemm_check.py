@@ -75,15 +75,11 @@ for (M, N, K) in [] if C3_ONLY else [(24196, 2048, 2048), (8192, 2048, 2048), (2
 # forward: per-tensor X and W, fp32 output + tile-scaled companion emitted (ReLU); data-grad: per-tensor dZ, ReLU mask from the hi
 # plane of that companion, fp32 output + emitted companion + column sums; weight-grad: both operands tile-scaled (the two emitted
 # companions) -- 128 CTAs of about 6,400 k-blocks each and no split, the mainloop alone.  Issued = 3 fp16 MMAs per product.
-def per_tensor_desc(h):
-    return native.H16Desc(h.buf.data_ptr(), h.amax.data_ptr(), h.ld, h.rows, h.cols, 0, 0, 0)
-
-
 def tiled_desc(rows, cols):
     ld = (cols + 7) // 8 * 8
     buf = torch.zeros(2, rows, ld, device=dev, dtype=torch.float16)
     amax = torch.zeros((rows + 127) // 128, (cols + 255) // 256, device=dev, dtype=torch.int32)
-    return native.H16Desc(buf.data_ptr(), amax.data_ptr(), ld, rows, cols, amax.shape[1], 1, 0), (buf, amax)
+    return ops.H16(buf, amax, rows, cols, ld, amax.shape[1], 1).desc(), (buf, amax)
 
 
 M, N, K = 206139, 2048, 2048
@@ -91,19 +87,19 @@ torch.manual_seed(0)
 x = torch.randn(M, K, device=dev); W = torch.randn(N, K, device=dev) / math.sqrt(K); b = torch.randn(N, device=dev) * 0.1
 dz = torch.randn(M, N, device=dev) * 1e-3
 xh, wh, dzh = ops.split_h(x), ops.split_h(W), ops.split_h(dz)
-X, Wd, DZ = per_tensor_desc(xh), per_tensor_desc(wh), per_tensor_desc(dzh)
+X, Wd, DZ = xh.desc(), wh.desc(), dzh.desc()
 y = torch.empty(M, N, device=dev); Yh, keep_y = tiled_desc(M, N)
 dx = torch.empty(M, K, device=dev); dXh, keep_dx = tiled_desc(M, K)
 colsum = torch.zeros(K, device=dev)
 dW = torch.empty(K, N, device=dev)
 st = _C.stream()
-f_fwd, f_dgrad, f_wgrad = native.fn('gcbf_linear_fwd_t'), native.fn('gcbf_linear_bwd_data_t'), native.fn('gcbf_linear_bwd_weight_t')
+f_fwd, f_dgrad, f_wgrad = native.fn('gcbf_linear_fwd_h'), native.fn('gcbf_linear_bwd_data_h'), native.fn('gcbf_linear_bwd_weight_h')
 products = {
     'fwd': lambda: native.check(f_fwd(ctypes.byref(X), ctypes.byref(Wd), _C.ptr(b), None, ops.ACT_RELU, _C.ptr(y), N, ctypes.byref(Yh), None,
-                                      M, N, K, st), 'fwd'),
+                                      M, N, K, st, 3), 'fwd'),
     'dgrad': lambda: native.check(f_dgrad(ctypes.byref(DZ), ctypes.byref(Wd), None, None, 0, ctypes.byref(Yh), _C.ptr(dx), K, 0,
-                                          ctypes.byref(dXh), _C.ptr(colsum), None, M, N, K, st), 'dgrad'),
-    'wgrad': lambda: native.check(f_wgrad(ctypes.byref(dXh), ctypes.byref(Yh), None, _C.ptr(dW), N, 0, M, K, N, st), 'wgrad'),
+                                          ctypes.byref(dXh), _C.ptr(colsum), None, M, N, K, st, 3), 'dgrad'),
+    'wgrad': lambda: native.check(f_wgrad(ctypes.byref(dXh), ctypes.byref(Yh), None, _C.ptr(dW), N, 0, M, K, N, st, 3), 'wgrad'),
 }
 fl = 2.0 * M * N * K
 res = {}
